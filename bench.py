@@ -15,8 +15,8 @@ every ready task is assigned in that one tick and value = tasks / tick time.
           between two kernel launches (--nccl-exchange).
 
   value     device-resident: the ready set already sits in HBM; the timed region holds K ticks on K different contexts
-            (K + W distinct 12-15 MB task tables > the 126 MB L2, so no step re-reads a warm table); a tick = ONE
-            cooperative kernel (histogram, solve, emit) that reads the worker state from pinned host memory.
+            (K + W distinct 12-15 MB task tables, more than the 50 MB L2 of an H100, so no step re-reads a warm table); a
+            tick = ONE cooperative kernel (histogram, solve, emit) that reads the worker state from pinned host memory.
   e2e       the same tick through the public C ABI with HOST buffers: hqs_ready_push (H2D of the task, class and
             priority arrays from pinned memory) + hqs_tick (D2H of the 8-byte assignments and the free vectors) inside
             the timed region.
@@ -26,6 +26,10 @@ every ready task is assigned in that one tick and value = tasks / tick time.
   cpu_baseline / --impl reference   the oracle (restated reference tick, HiGHS 1.12.0) on the SAME workload, single-
             threaded like the reference (Rc<RefCell<Core>>), with the reference's solver defaults relaxed to a 1 % MIP gap
             and a 2 s cap (parity.ORACLE_FAST; `solver_hit_cap` says whether the cap was reached).
+
+--dump-outputs DIR writes what the last timed step returned to its caller (the assignment records, field by field, and
+the free vectors after the tick) as DIR/<name>.npy.  The inputs depend only on the arguments, so two builds can be
+compared output for output.
 """
 from __future__ import annotations
 
@@ -65,11 +69,12 @@ def _peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
 
 
 class ClockSampler(threading.Thread):
-    """Samples nvidia-smi clocks and throttle reasons while the timed region runs."""
+    """Samples nvidia-smi clocks and throttle reasons while the timed region runs; records the card's name and power
+    limit, which belong beside every number the run reports."""
 
     def __init__(self, index: int = 0) -> None:
         super().__init__(daemon=True)
@@ -77,9 +82,17 @@ class ClockSampler(threading.Thread):
         self.samples = []
         self.reasons = set()
         self.sm_max = None
+        self.gpu, self.power_limit_w = None, None
         self._halt = threading.Event()
 
     def run(self) -> None:
+        try:
+            out = subprocess.run(["nvidia-smi", f"--id={self.index}", "--query-gpu=name,power.limit",
+                                  "--format=csv,noheader,nounits"], capture_output=True, text=True, timeout=5).stdout
+            name, limit = [x.strip() for x in out.strip().split(",")]
+            self.gpu, self.power_limit_w = name, float(limit)
+        except Exception:
+            pass
         q = ("clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
              "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
@@ -100,7 +113,8 @@ class ClockSampler(threading.Thread):
     def stop(self) -> dict:
         self._halt.set()
         self.join(timeout=6)
-        return {"sm_mhz": float(np.median(self.samples)) if self.samples else None, "sm_max_mhz": self.sm_max,
+        return {"gpu": self.gpu, "power_limit_w": self.power_limit_w,
+                "sm_mhz": float(np.median(self.samples)) if self.samples else None, "sm_max_mhz": self.sm_max,
                 "reasons": sorted(self.reasons), "samples": len(self.samples)}
 
 
@@ -251,6 +265,18 @@ def drain(P, wl, device: int, max_ticks: int = 20000, dag: bool = False):
             "ms_per_tick": 1000.0 * dt / max(ticks, 1), "assigned": wl.n_tasks - left}
 
 
+def dump_outputs(out_dir: str, assignments: np.ndarray, free_after: np.ndarray, rank) -> None:
+    """Writes one step's result as the caller of the tick receives it: the assignment records in output order, one
+    array per field, and the free vectors [W][R] after the tick.  Task ids and amounts stay below 2^53, so float64 holds
+    them exactly (about 32 MB at 1 M assignments)."""
+    os.makedirs(out_dir, exist_ok=True)
+    prefix = "" if rank is None else f"rank{rank}_"
+    arrays = {f"assignment_{f}": assignments[f] for f in assignments.dtype.names}
+    arrays["free_after"] = free_after
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{prefix}{name}.npy"), np.ascontiguousarray(a, dtype=np.float64))
+
+
 def run_cuda(args) -> dict:
     import torch
     import torch.distributed as dist
@@ -393,12 +419,16 @@ def run_cuda(args) -> dict:
         scheds[i]._check(lib.hqs_tick_fetch(scheds[i]._ctx, n_tasks, L.ptr(tmp_out), C.byref(out_n), None))
     # every step must have assigned every task of the rank
     n_done_local = 0
+    last_free_after = np.zeros_like(wl.worker_free)
     for i in range(K):
         s = scheds[Wm + i]
-        s._check(lib.hqs_tick_fetch(s._ctx, n_tasks, L.ptr(tmp_out), C.byref(out_n), None))
+        s._check(lib.hqs_tick_fetch(s._ctx, n_tasks, L.ptr(tmp_out), C.byref(out_n),
+                                    L.ptr(last_free_after) if i == K - 1 else None))
         n_done_local = int(out_n.value)
         if world == 1:
             assert out_n.value == n_tasks, f"step {i}: {out_n.value} of {n_tasks} tasks assigned"
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, tmp_out[: out_n.value], last_free_after, rank if world > 1 else None)
 
     if world > 1:
         t = torch.tensor([ms_total], dtype=torch.float64, device=dev)
@@ -434,14 +464,8 @@ def run_cuda(args) -> dict:
     bytes_interned = BYTES_INTERNED * n_tasks + worker_bytes
     kernel_ms = ms_per_step if (world == 1 or p2p) else float(acc[3])
     achieved = bytes_contract / kernel_ms / 1e6
-    traffic = None          # dram read + write bytes of one tick_k launch from the committed ncu --set full capture
-    mp = os.path.join(ROOT, "profiles", "r2_ncu_metrics.json")
-    if os.path.exists(mp):
-        m = json.load(open(mp)).get("tick_k")
-        if m and m.get("dram_bytes_read") is not None:
-            traffic = m["dram_bytes_read"] + (m.get("dram_bytes_write") or 0.0)
     roofline = {"bound": "hbm", "kernel": "tick_k (the one kernel of a tick: histogram + solve + emit)", "achieved": achieved,
-                "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": traffic, "peak_source": peak_src,
+                "peak": peak, "unit": "GB/s", "frac": achieved / peak, "peak_source": peak_src,
                 "bytes_per_assignment": BYTES_CONTRACT,
                 "algorithmic_bytes_per_launch": bytes_contract,
                 "kernel_ms": kernel_ms,
@@ -496,7 +520,7 @@ def run_cuda(args) -> dict:
     h_cls, h_prio = pin(wl.task_class), pin(prio)
     out = torch.empty(n_tasks * 8, dtype=torch.uint8).pin_memory().numpy().view(L.assignment_dtype)
     free_after = np.zeros_like(free)
-    n_e2e = max(3, min(K, 10))
+    n_e2e = K
 
     def e2e_step():
         # the rank's tasks are one task array (consecutive handles): class ids and priorities cross PCIe, the handles do not
@@ -552,7 +576,7 @@ def run_cuda(args) -> dict:
             "config": config_block(cfg, world, all_assigned=bool(n_per_step == world * n_tasks),
                                    exchange=("p2p" if p2p else ("nccl" if world > 1 else "none")),
                                    l2_policy=f"each timed step runs on a different task table (K+W tables x {12 * n_tasks // 1_000_000} MB "
-                                             "> 126 MB L2): inputs larger than L2",
+                                             f"> {torch.cuda.get_device_properties(dev).L2_cache_size >> 20} MB L2): inputs larger than L2",
                                    host_wall_ms_per_step=1000.0 * t_host / K),
             "gpu_launches": launches_timed, "clocks": clocks, "e2e": e2e, "roofline": roofline, "kernels": kernels,
             "cpu_baseline": cpu, "extra": extra,
@@ -578,7 +602,11 @@ def main() -> None:
     ap.add_argument("--no-drain", action="store_true", help="alias of --no-extras")
     ap.add_argument("--nccl-exchange", action="store_true",
                     help="N > 1: all-gather the count vectors with NCCL instead of the fused peer-to-peer exchange")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's assignments and free vectors to DIR/<name>.npy (float64)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     args.no_extras = args.no_extras or args.no_drain
     args.warmup = max(args.warmup, 3) if args.impl == "cuda" else args.warmup
     rank = int(os.environ.get("RANK", "0"))

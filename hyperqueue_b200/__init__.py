@@ -1,4 +1,4 @@
-"""hyperqueue_b200 — B200-native task->worker assignment solver for HyperQueue's tako scheduler tick.
+"""hyperqueue_b200 — H100-native (sm_90a) task->worker assignment solver for HyperQueue's tako scheduler tick.
 
 Only the hot path is here (SURVEY.md §8): the CUDA kernels + C ABI (csrc/hqsched.cu, include/hqsched.h)
 and a thin host-side mirror of tako's scheduler seam (scheduler.py).  There is no CPU fallback: every

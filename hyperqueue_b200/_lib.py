@@ -92,7 +92,7 @@ def load_library() -> C.CDLL:
     if _lib is not None:
         return _lib
     if not os.path.exists(LIB_PATH):
-        raise LibraryNotBuilt(f"{LIB_PATH} is missing: run `python __graft_entry__.py` (nvcc, sm_100a). "
+        raise LibraryNotBuilt(f"{LIB_PATH} is missing: run `python __graft_entry__.py` (nvcc, sm_90a). "
                               "hyperqueue_b200 has no CPU fallback.")
     lib = C.CDLL(LIB_PATH)
     vp, u32, u64p, u32p, u8p = C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p

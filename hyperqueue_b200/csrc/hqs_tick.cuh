@@ -22,7 +22,7 @@
 
 constexpr u32 TICK_THREADS = 512;
 constexpr u32 TICK_WARPS = TICK_THREADS / 32;
-constexpr u32 EMIT_ROWS_MAX = 20;     // rows of 32 tasks per emit warp and chunk (1.5 M table slots are one chunk per worker CTA)
+constexpr u32 EMIT_ROWS_MAX = 20;     // rows of 32 tasks per emit warp and chunk (1.34 M table slots are one chunk per worker CTA on 132 SMs)
 constexpr u32 EMIT_SEG_SMEM = 1024;   // count segments cached in shared memory by the emit step
 constexpr u32 CMD_PACK = 1, CMD_EMIT = 2, CMD_EXIT = 3;      // grid commands: cmd word = (sequence << 2) | type
 constexpr u32 BLK_PACK = 1, BLK_RESTART = 2, BLK_END = 3, BLK_PREFILL = 4, BLK_WIDE = 5;    // block commands inside the solver CTA

@@ -1,4 +1,4 @@
-// hqsched.cu — B200 (sm_100a) task->worker assignment solver behind the C ABI of include/hqsched.h.
+// hqsched.cu — H100 (sm_90a) task->worker assignment solver behind the C ABI of include/hqsched.h.
 //
 // Replaces, for the single-node hot path of HyperQueue's tako scheduler tick (v0.26.0):
 //   create_task_batches        crates/tako/src/internal/scheduler/batches.rs:42-181   (priority histogram)
@@ -110,8 +110,8 @@ struct hqs_ctx {
     u32 push_cap = 0;
     u32* d_newcnt = nullptr; u64* d_newprio = nullptr;
     // tick buffers
-    u32 sm_count = 148;
-    u32 grid_ctas = 148;                // CTAs of the cooperative tick kernel (solver CTA + worker CTAs)
+    u32 sm_count = 132;
+    u32 grid_ctas = 132;                // CTAs of the cooperative tick kernel (solver CTA + worker CTAs)
     u32 G_cap = 0, P_cap = 0;
     u32* d_table = nullptr;
     u32* d_total = nullptr;
@@ -769,7 +769,7 @@ int hqs_create(hqs_ctx** out, int device, uint32_t n_resources, uint32_t flags) 
         delete ctx;
         return HQS_E_CUDA;
     }
-    ctx->sm_count = sms > 0 ? (u32)sms : 148;
+    ctx->sm_count = sms > 0 ? (u32)sms : 132;
     // one CTA per SM (cooperative launch: all CTAs are co-resident).  HQS_CREATE_SHARE_DEVICE: half of the SMs, so
     // that two contexts whose ticks wait for each other on the device (peer exchange) can run side by side on one GPU
     ctx->grid_ctas = std::max<u32>(2, (flags & 4u) ? ctx->sm_count / 2 : ctx->sm_count);

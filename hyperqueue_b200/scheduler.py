@@ -1,7 +1,7 @@
 """Host-side mirror of tako's scheduler seam over the C ABI (include/hqsched.h).
 
 What the Rust shim of INTEGRATION.md does inside `run_scheduling_inner`
-(/root/reference/crates/tako/src/internal/scheduler/main.rs:40-46) is done here in Python so that the
+(hyperqueue/crates/tako/src/internal/scheduler/main.rs:40-46) is done here in Python so that the
 parity tests and the benchmark read like the reference's own tests:
 
   reference (Rust)                                          here

@@ -1,5 +1,5 @@
 /*
- * hqsched.h — C ABI of the B200-native task->worker assignment solver (libhqsched_b200.so).
+ * hqsched.h — C ABI of the H100-native (sm_90a) task->worker assignment solver (libhqsched_b200.so).
  *
  * Drop-in boundary for the hot path of HyperQueue's tako scheduler tick (v0.26.0).  The reference has
  * no FFI for this path; the seam it replaces is the pair

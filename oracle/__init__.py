@@ -4,8 +4,8 @@ TEST INFRASTRUCTURE ONLY.  Nothing under ``hyperqueue_b200/`` may import this pa
 ``tests/``, ``__graft_entry__.smoke()`` and ``bench.py``'s CPU-baseline / ``--impl reference``
 legs use it, and there only as the checker (or as the timed CPU baseline), never as the product.
 
-The reference is Rust + HiGHS (crate ``highs 1.12.0`` / ``highs-sys 1.12.1``, not vendored under
-/root/reference) and cannot be built in this image (no cargo/rustc).  This package restates the
+The reference is Rust + HiGHS (crate ``highs 1.12.0`` / ``highs-sys 1.12.1``, not vendored in the
+reference repository) and is not built here (it needs cargo/rustc).  This package restates the
 algorithm in Python/numpy, solving the MIP with the same HiGHS version (1.12.0) bundled in scipy
 (``scipy.optimize.milp``).  Parity is PINNED: ``tests/test_oracle_golden.py`` replays the
 known-answer vectors of the reference's own tests

@@ -1,6 +1,6 @@
 """Task batches and priority cuts, restated (TEST INFRASTRUCTURE — see oracle/__init__.py).
 
-Follows /root/reference/crates/tako/src/internal/scheduler/batches.rs:
+Follows hyperqueue/crates/tako/src/internal/scheduler/batches.rs:
   :8-9      BATCH_PRUNING_MAX_SIZE = 32, BATCH_PRUNING_FIXED_PREFIX = 4
   :11-40    PriorityCut {size, blockers[(rq, Some(size)|None)]}, TaskBatch {rq, cuts, size, limit,
             limit_reached, is_blocker}

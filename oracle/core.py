@@ -1,6 +1,6 @@
 """Server core state and the tick driver, restated (TEST INFRASTRUCTURE — see oracle/__init__.py).
 
-Follows (paths relative to /root/reference/crates/tako/src/internal/):
+Follows (paths relative to hyperqueue/crates/tako/src/internal/):
   server/core.rs:41-62 (Core), :207-235 (add_task / remove_task)
   server/task.rs:22-43,115-125,175-177     Task, TaskRuntimeState, priority()
   server/reactor.rs:188-220                on_new_tasks (dependency counting, ready insertion)

@@ -1,7 +1,7 @@
 """Gap computation ("how many low-priority tasks still fit beside a maximally packed high-priority
 class"), restated (TEST INFRASTRUCTURE — see oracle/__init__.py).
 
-Follows /root/reference/crates/tako/src/internal/scheduler/gap.rs:
+Follows hyperqueue/crates/tako/src/internal/scheduler/gap.rs:
   :37-93    GapCache::get_gap
   :96-147   compute_gap_resources (one small LP per non-zero worker resource)
 Pinned by the 13 asserts of gap.rs:175-246 (tests/test_oracle_golden.py::test_compute_gap).

@@ -1,7 +1,7 @@
 /* Plain-C restatement of the per-(worker, class, variant) admission predicate and the per-(worker,
  * resource) capacity check (TEST INFRASTRUCTURE — see oracle/__init__.py and oracle/judge.py).
  *
- * Follows /root/reference/crates/tako/src/internal/
+ * Follows hyperqueue/crates/tako/src/internal/
  *   scheduler/solver.rs:103-105      !blocked && has_time_to_run && have_immediate_resources_for_rq
  *   server/workerload.rs:77-83       is_capable_to_run_request: every entry's min_amount <= free
  *   common/resources/request.rs:34-36  min_amount of `All` is one fraction

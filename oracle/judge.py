@@ -5,7 +5,7 @@ check": this module restates exactly that check, independent of any scheduler:
 
   per (worker, class, variant)   the solver's admission predicate
       !is_request_blocked && has_time_to_run && have_immediate_resources_for_rq
-      (/root/reference/crates/tako/src/internal/scheduler/solver.rs:103-105,
+      (hyperqueue/crates/tako/src/internal/scheduler/solver.rs:103-105,
        server/worker.rs:273-278,320-326,328-334, server/workerload.rs:77-83;
        `All` needs 1 fraction: common/resources/request.rs:34-36)
   per (worker, resource)         the capacity row  sum cap * x <= free   with cap = amount, or the

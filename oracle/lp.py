@@ -1,11 +1,11 @@
 """LP/MIP facade over HiGHS, restated (TEST INFRASTRUCTURE — see oracle/__init__.py).
 
-Follows /root/reference/crates/tako/src/internal/solver/mod.rs:27-41 (LpInnerSolver trait) and
+Follows hyperqueue/crates/tako/src/internal/solver/mod.rs:27-41 (LpInnerSolver trait) and
 solver/highs.rs:4-63 (HiGHS backend: integer columns 0..=1 / 0.., rows `..=v`, `v..`, `v..=v`,
 `optimise(Sense::Maximise).solve()`, result only when HighsModelStatus::Optimal).
 
 The reference links HiGHS through crate `highs 1.12.0` / `highs-sys 1.12.1` (Cargo.lock:1106-1123,
-source not under /root/reference).  Here the same HiGHS release (1.12.0, bundled in scipy 1.18) is
+source not in the reference repository).  Here the same HiGHS release (1.12.0, bundled in scipy 1.18) is
 driven through scipy.optimize.milp.  Among tied optima the two drivers may differ (option defaults
 of the `highs` crate are not verifiable here); the reference's own tests tolerate that (eq_class).
 """

@@ -1,7 +1,7 @@
 """Counts -> concrete (task, worker, variant) mapping and proactive prefilling, restated
 (TEST INFRASTRUCTURE — see oracle/__init__.py).
 
-Follows /root/reference/crates/tako/src/internal/scheduler/mapping.rs:
+Follows hyperqueue/crates/tako/src/internal/scheduler/mapping.rs:
   :9-21     WorkerTaskUpdate {assigned[(task, variant)], prefills, retracts}, WorkerTaskMapping
   :23-154   create_task_mapping (take_tasks(sum), one task per worker per pass, state machine
             Waiting->Assigned / Prefilled->Retracting(+retract+redirect) / Retracting->redirect update,

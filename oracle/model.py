@@ -1,6 +1,6 @@
 """Resource model of the tako scheduler, restated (TEST INFRASTRUCTURE — see oracle/__init__.py).
 
-Follows (paths relative to /root/reference/crates/tako/src/internal/):
+Follows (paths relative to hyperqueue/crates/tako/src/internal/):
   common/resources/amount.rs:7,26-104      ResourceAmount: u64 fixed point, 10 000 fractions per unit
   common/resources/request.rs:13-83        AllocationRequest (6 policies, `All` has no amount)
   common/resources/request.rs:107-134      ResourceWeight (u32, x10 000)

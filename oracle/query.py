@@ -1,6 +1,6 @@
 """Autoalloc what-if query, restated (TEST INFRASTRUCTURE — see oracle/__init__.py).
 
-Follows /root/reference/crates/tako/src/internal/scheduler/query.rs:
+Follows hyperqueue/crates/tako/src/internal/scheduler/query.rs:
   :12-70    fake workers per WorkerTypeQuery (partial descriptors get ResourceAmount::MAX for every resource
             the query does not name)
   :72-95    create_task_batches + run_scheduling_solver over the FAKE workers only; a fake worker is "needed" iff

@@ -1,6 +1,6 @@
 """The MILP scheduling solver, restated (TEST INFRASTRUCTURE — see oracle/__init__.py).
 
-Follows /root/reference/crates/tako/src/internal/scheduler/solver.rs:
+Follows hyperqueue/crates/tako/src/internal/scheduler/solver.rs:
   :10-14    SchedulingSolution {sn_counts[(rq, variant)][worker] = u32}
   :16-62    worker list (sn-capable, sorted by id), resource_sums (MAX counts as 1.0)
   :75-174   per worker: placement variables for every feasible (batch, variant), reservation

@@ -1,6 +1,6 @@
 """Ready-task queues per request class, restated (TEST INFRASTRUCTURE — see oracle/__init__.py).
 
-Follows /root/reference/crates/tako/src/internal/scheduler/taskqueue.rs:
+Follows hyperqueue/crates/tako/src/internal/scheduler/taskqueue.rs:
   :26-72    TaskQueues (one TaskQueue per ResourceRqId; add_ready_task disposes lower-priority prefills)
   :114-119  TaskQueue {queue: BTreeMap<Reverse<Priority>, OneOrMoreTaskIds>, prefill: Option<(Priority, Set)>}
   :146-152  check_dispose_prefill

@@ -1,6 +1,6 @@
 """Test DSL over the oracle, mirroring the reference's own test helpers so that the golden vectors can
 be transcribed one to one:
-  /root/reference/crates/tako/src/internal/tests/utils/env.rs        TestEnv (worker ids from 50, task ids from 1)
+  hyperqueue/crates/tako/src/internal/tests/utils/env.rs        TestEnv (worker ids from 50, task ids from 1)
   .../tests/utils/task.rs        TaskBuilder     .../tests/utils/worker.rs   WorkerBuilder
   .../tests/utils/resources.rs   ResBuilder (adds 1 cpu if no cpu entry: resources.rs:99-109)
   .../tests/utils/scheduler.rs   TestCase (expect_tasks / expect_request_v / eq_class / running_c)

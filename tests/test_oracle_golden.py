@@ -1,7 +1,7 @@
 """Pins the oracle against the reference's own known-answer vectors (SURVEY.md Appendix B).
 
 Every test below is a transcription of a test in
-/root/reference/crates/tako/src/internal/tests/test_scheduler_sn.rs (line ranges in each docstring),
+hyperqueue/crates/tako/src/internal/tests/test_scheduler_sn.rs (line ranges in each docstring),
 scheduler/gap.rs:175-246 or scheduler/batches.rs:223-250.  CPU only.
 """
 import pytest

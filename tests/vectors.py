@@ -3,7 +3,7 @@ through the sequential specification (CPU) and the CUDA path (GPU).
 
 Each case: workers (cpus[, extra resources]), tasks (priority, request variants), expected per-worker result as
 a multiset of (class key, variant) counts — or None where only a predicate is pinned.  Source lines refer to
-/root/reference/crates/tako/src/internal/tests/test_scheduler_sn.rs.
+hyperqueue/crates/tako/src/internal/tests/test_scheduler_sn.rs.
 """
 from __future__ import annotations
 

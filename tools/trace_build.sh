@@ -3,5 +3,5 @@
 # of the lean first-fit loop (tools/trace_probe.py reads them).  The product library is not touched.
 set -e
 cd "$(dirname "$0")/.."
-nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -std=c++17 -DHQS_TRACE -Xcompiler -fPIC,-Wall,-Wno-subobject-linkage \
+nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 -DHQS_TRACE -Xcompiler -fPIC,-Wall,-Wno-subobject-linkage \
      --shared -cudart shared -Iinclude -o hyperqueue_b200/libhqsched_b200_trace.so hyperqueue_b200/csrc/hqsched.cu

@@ -4,5 +4,5 @@
 set -e
 cd "$(dirname "$0")/.."
 sfx=$1; shift
-nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo -O3 -std=c++17 "$@" -Xcompiler -fPIC,-Wall,-Wno-subobject-linkage \
+nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 "$@" -Xcompiler -fPIC,-Wall,-Wno-subobject-linkage \
      --shared -cudart shared -Iinclude -o hyperqueue_b200/libhqsched_b200_$sfx.so hyperqueue_b200/csrc/hqsched.cu
