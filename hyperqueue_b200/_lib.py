@@ -58,7 +58,12 @@ class hqs_stats(C.Structure):
     _fields_ = [("n_groups", C.c_uint32), ("n_levels", C.c_uint32), ("n_assigned", C.c_uint32),
                 ("n_segments", C.c_uint32), ("kernel_launches", C.c_uint64), ("ticks", C.c_uint64),
                 ("n_handles", C.c_uint32), ("coarsened", C.c_uint32),
-                ("narrow_amounts", C.c_uint32), ("reserved", C.c_uint32)]
+                ("narrow_amounts", C.c_uint32), ("solver_path", C.c_uint32)]
+
+
+# hqs_stats.solver_path bits (include/hqsched.h)
+HQS_PATH_WIDE, HQS_PATH_LEAN, HQS_PATH_LEAN_EXTRAS, HQS_PATH_GENERAL = 0x01, 0x02, 0x04, 0x08
+HQS_PATH_PACKED, HQS_PATH_MU_RESTART, HQS_PATH_CLASSES_GLOBAL, HQS_PATH_REM_GLOBAL = 0x10, 0x20, 0x40, 0x80
 
 
 worker_dtype = np.dtype([("worker_id", "<u4"), ("flags", "<u4"), ("remaining_time_ms", "<u8"),

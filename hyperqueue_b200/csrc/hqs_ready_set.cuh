@@ -31,6 +31,8 @@ struct TickHeaderOut {
     u32 error;       // 1 = segment overflow, 2 = a grid wait timed out, 3 = out_cap too small (nothing was emitted)
     u32 n_prefilled; // prefill records (kind 1) behind the assignments
     u32 pad;         // detail of error 2: which wait timed out
+    u32 solver_path; // HQS_PATH_* bits: which solve loops ran (hqs_stats.solver_path)
+    u32 pad2;
     unsigned long long dbg[8];   // clock64 phase lengths of the solver CTA (hqs_debug_read)
 };
 

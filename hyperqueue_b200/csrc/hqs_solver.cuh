@@ -1,7 +1,7 @@
 // hqs_solver.cuh — device-side building blocks of the tick: the class table layout, the exact fit count
 // (how many tasks of a request fit into a free vector), the pack step (one warp fills one worker) and the
-// acquire/release helpers.  Included by hqsched.cu inside its anonymous namespace; the tick kernel itself
-// is hqs_tick.cuh.
+// acquire/release helpers, and the host code that packs a variant into its device record.  Included by hqsched.cu inside
+// its anonymous namespace (and by the fit-count probe of the tests); the tick kernel itself is hqs_tick.cuh.
 #pragma once
 
 constexpr u32 PACK_MAX_CAND = 64;    // (class, variant) candidates of the packed level: 2 per lane
@@ -37,6 +37,65 @@ template <typename AT> struct AmountMax;
 template <> struct AmountMax<u64> { static constexpr u64 value = HQS_AMOUNT_MAX; };
 template <> struct AmountMax<u32> { static constexpr u32 value = 0xFFFFFFFFu; };
 constexpr u64 NARROW_LIMIT = 0x7FFFFFFFull;      // scaled amounts of the narrow path stay below 2^31
+
+// ---- host: one ABI variant -> its device record (hqs_classes_set; the fit-count probe of the tests uses the same code).
+// The caller has checked that the variant requests no resource >= R.
+template <int RT>
+inline void pack_var64(VarT<RT, u64>& dv, const hqs_variant& hv, u32 R) {
+    u32 used = 0;
+    for (u32 r = 0; r < R; ++r) {
+        const bool all = (hv.all_mask >> r) & 1;
+        const u64 amt = hv.amount[r];
+        dv.amount[r] = all ? 0 : amt;
+        dv.rcpf[r] = (!all && amt) ? 1.0f / (float)amt : 0.0f;
+        dv.rcpf[RT + r] = all ? 0.0f : (float)(double)amt;          // u64 -> double -> float, both RN
+        if (all || amt) used |= 1u << r;
+    }
+    dv.min_time_ms = hv.min_time_ms;
+    dv.all_mask = hv.all_mask & ((1u << R) - 1);
+    dv.used_mask = used;
+}
+
+// Magic number and shifts of the division by the invariant amount 1 <= d < 2^32 (see fit_count):
+// l = ceil(log2 d), m = floor(2^32 (2^l - d) / d) + 1, sh = min(l, 1) | max(l - 1, 0) << 1.
+inline void div_magic(u32 d, u32* magic, u32* sh) {
+    u32 l = 0;
+    while (l < 32 && ((u64)1 << l) < d) ++l;
+    *magic = (u32)((((u64)1 << 32) * (((u64)1 << l) - d)) / d + 1);
+    *sh = (l < 1 ? l : 1) | ((l > 0 ? l - 1 : 0) << 1);
+}
+
+// The narrow record: amounts divided by the per-resource gcd `gscale` (which divides every requested amount).  Returns
+// false if a scaled amount does not fit the narrow path (> NARROW_LIMIT); the record is then not usable.
+template <int RT>
+inline bool pack_var32(VarT<RT, u32>& dv, const hqs_variant& hv, u32 R, const u64* gscale) {
+    bool ok = true;
+    u32 used = 0;
+    unsigned char* shb = reinterpret_cast<unsigned char*>(dv.shw);         // one byte per resource
+    for (u32 r = 0; r < R; ++r) {
+        const bool all = (hv.all_mask >> r) & 1;
+        const u64 amt = all ? 0 : hv.amount[r] / gscale[r];
+        if (amt > NARROW_LIMIT) ok = false;
+        dv.amount[r] = (u32)amt;
+        if (amt && amt <= NARROW_LIMIT) {
+            u32 magic, sh;
+            div_magic((u32)amt, &magic, &sh);
+            memcpy(&dv.rcpf[r], &magic, 4);
+            shb[r] = (unsigned char)sh;
+        } else {
+            dv.rcpf[r] = 0.0f;
+        }
+        dv.rcpf[RT + r] = all ? 0.0f : (float)(double)hv.amount[r];
+        if (all || hv.amount[r]) used |= 1u << r;
+    }
+    dv.min_time_ms = hv.min_time_ms;
+    dv.all_mask = hv.all_mask & ((1u << R) - 1);
+    dv.used_mask = used;
+    return ok;
+}
+
+#ifdef __CUDACC__
+// ---- device side (everything below; a host-only compiler sees the layouts and the packing helpers above)
 
 struct PackScratch {          // global memory, written by the solver CTA, read by the pack warps (and back)
     u64* fr;                  // [W][R]
@@ -96,11 +155,13 @@ __device__ __forceinline__ u64 fit_count(const u64 (&fr)[RT], u32 untouched, con
         // the 64-bit free amount is converted through its 32-bit halves (fp64 and 64-bit divisions cost hundreds of cycles)
         const float nf = __fmaf_rn(__uint2float_rn((u32)(n >> 32)), 4294967296.0f, __uint2float_rn((u32)n));
         const float qf = nf * dv.rcpf[r];
+        // the fix-ups compare the full 128-bit product: near 2^64 the estimate can be 2^64 / d (nf rounds up to 2^64),
+        // q * d then wraps, and a wrapped product would read as "fits" and over-count
         u64 q = (u64)__float2uint_rz(fminf(qf, 1048576.0f));
         u64 p = q * d;
-        q = p > n ? q - 1 : (n - p >= d ? q + 1 : q);
+        q = (__umul64hi(q, d) != 0 || p > n) ? q - 1 : (n - p >= d ? q + 1 : q);
         p = q * d;
-        q = p > n ? q - 1 : (n - p >= d ? q + 1 : q);
+        q = (__umul64hi(q, d) != 0 || p > n) ? q - 1 : (n - p >= d ? q + 1 : q);
         const u64 q_all = (untouched >> r) & 1;
         const bool unconstrained = !on || (!all && (n == HQS_AMOUNT_MAX || fits_cap));
         big |= on && !all && !unconstrained && qf >= 1048576.0f;
@@ -318,3 +379,4 @@ __device__ void pack_body(const PackArgs& a, unsigned char* smem_dyn) {
         }
     }
 }
+#endif  // __CUDACC__

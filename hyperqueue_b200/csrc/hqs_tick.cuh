@@ -1259,6 +1259,8 @@ __device__ void solver_cta(const TickArgs& a, unsigned char* smem) {
     // =============================================================================================
     u32 n_assigned = 0, n_segments = 0, n_visits = 0, n_fast = 0;
     long long t_pack = 0, t_general = 0;      // cycles inside pack commands / the general first-fit loop (hqs_debug_read)
+    // HQS_PATH_* bits of the header (hqs_stats.solver_path): where the solve's data lives, then the loops the solver warp ran
+    u32 path = (a.sm.classes == SM_NONE ? HQS_PATH_CLASSES_GLOBAL : 0u) | (NARROW && a.sm.rem == SM_NONE ? HQS_PATH_REM_GLOBAL : 0u);
 #ifdef HQS_TRACE
     // measuring build (tools/trace_build.sh): cycle sums of the sections of the lean loop replace the phase stamps
     u32 tr_top = 0, tr_rec = 0, tr_cyc[4] = {0, 0, 0, 0}, tr_n[4] = {0, 0, 0, 0}, tr_fit = 0, tr_load = 0;   // visit kinds: dead tile, fall, scan (tile exhausted), scan (group ends)
@@ -1362,6 +1364,7 @@ __device__ void solver_cta(const TickArgs& a, unsigned char* smem) {
                             t_pack += clock64() - tp0;
                             packed = true;
                             level_packed = s_err == 0;
+                            if (level_packed) path |= HQS_PATH_PACKED;
                         }
                     }
                 }
@@ -1548,8 +1551,9 @@ __device__ void solver_cta(const TickArgs& a, unsigned char* smem) {
                             }
                         }
                     };
-                    if (resv_on || s_kk) lean_loop(std::true_type{});
+                    if (resv_on || s_kk) { lean_loop(std::true_type{}); path |= HQS_PATH_LEAN_EXTRAS; }
                     else if (wide_ok) {
+                        path |= HQS_PATH_WIDE;
                         // every worker a lane: all warps of the CTA (see wide_loop)
                         if (lane == 0) { s_blk[0] = BLK_WIDE; s_blk[1] = li; s_blk[2] = out_base; s_blk[3] = seg_base; }
                         __syncwarp();
@@ -1558,7 +1562,7 @@ __device__ void solver_cta(const TickArgs& a, unsigned char* smem) {
                         seg_base = wo.seg_base; out_base = wo.out_base;
                         seg_overflow |= wo.overflow;
                         n_visits += wo.steps;
-                    } else lean_loop(std::false_type{});
+                    } else { lean_loop(std::false_type{}); path |= HQS_PATH_LEAN; }
                     __syncwarp();
                     n_fast += n_list - li;
                     li = n_list;
@@ -1566,6 +1570,7 @@ __device__ void solver_cta(const TickArgs& a, unsigned char* smem) {
                 }
                 // ---- the groups of the level, in order: first-fit (after what pack placed)
                 const long long tg0 = clock64();
+                path |= HQS_PATH_GENERAL;
                 u32 region_end = seg_base;
                 if (level_packed) {
                     region_end = seg_base + 2u * W * s_cbase[ng];
@@ -1785,6 +1790,7 @@ __device__ void solver_cta(const TickArgs& a, unsigned char* smem) {
             }
             if (!__any_sync(0xffffffffu, viol)) break;
             // every listed group rewrites its record in the next pass
+            path |= HQS_PATH_MU_RESTART;
             if (lane == 0) s_blk[0] = BLK_RESTART;
             __syncwarp();
             bar_named(1, TICK_THREADS);
@@ -1846,6 +1852,8 @@ __device__ void solver_cta(const TickArgs& a, unsigned char* smem) {
         h.error = err;
         h.n_prefilled = s_npref;
         h.pad = s_err ? s_err : (werr ? 25u : 0u);       // which wait timed out (21 histogram, 22 | peer << 8, 23 pack, 24 emit, 25 a worker CTA)
+        h.solver_path = path;
+        h.pad2 = 0;
         h.dbg[0] = (unsigned long long)(t_counted - t_start);     // staging + wait for the histogram
         h.dbg[1] = (unsigned long long)(t_prologue - t_counted);  // exchange + compaction + demand
         h.dbg[2] = (unsigned long long)(t_solved - t_prologue);   // the solver warp

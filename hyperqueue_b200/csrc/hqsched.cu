@@ -689,6 +689,7 @@ int wait_header(hqs_ctx* ctx, TickHeaderOut* hdr) {
     ctx->stats.n_levels = ctx->last_L;
     ctx->stats.n_assigned = hdr->n_assigned;
     ctx->stats.n_segments = hdr->n_segments;
+    ctx->stats.solver_path = hdr->solver_path;
     memcpy(ctx->dbg, hdr->dbg, sizeof ctx->dbg);
     if (ctx->profile && ctx->ev_valid) {
         float ms = 0;
@@ -825,29 +826,17 @@ int hqs_classes_set(hqs_ctx* ctx, uint32_t n_classes, const hqs_class* classes) 
         unsigned char* cb = blob.data() + (size_t)c * cls_bytes;
         memcpy(cb, &sc.n_variants, 4);
         for (u32 v = 0; v < sc.n_variants; ++v) {
-            unsigned char* vb = cb + 8 + (size_t)v * var_bytes;
-            u64* amount = reinterpret_cast<u64*>(vb);
-            float* rcp = reinterpret_cast<float*>(vb + (size_t)RT * 8);
-            u64* min_time = reinterpret_cast<u64*>(vb + (size_t)RT * 16);
-            u32* masks = reinterpret_cast<u32*>(vb + (size_t)RT * 16 + 8);
-            u32 used = 0;
-            for (u32 r = 0; r < HQS_MAX_RESOURCES; ++r) {
-                const bool all = (sc.variants[v].all_mask >> r) & 1;
-                const u64 amt = sc.variants[v].amount[r];
-                if ((all || amt) && r >= ctx->R)
+            const hqs_variant& hv = sc.variants[v];
+            for (u32 r = ctx->R; r < HQS_MAX_RESOURCES; ++r)
+                if (((hv.all_mask >> r) & 1) || hv.amount[r])
                     return fail(ctx, HQS_E_INVALID, "class %u variant %u uses resource %u >= n_resources", c, v, r);
-                if (r < RT) {
-                    amount[r] = all ? 0 : amt;
-                    rcp[r] = (!all && amt) ? 1.0f / (float)amt : 0.0f;
-                    rcp[RT + r] = all ? 0.0f : (float)(double)amt;          // u64 -> double -> float, both RN
-                }
-                if (all || amt) used |= 1u << r;
-            }
+            unsigned char* vb = cb + 8 + (size_t)v * var_bytes;
+            u32 used;
+            if (RT == 4) { pack_var64<4>(*reinterpret_cast<VarT<4>*>(vb), hv, ctx->R); used = reinterpret_cast<VarT<4>*>(vb)->used_mask; }
+            else if (RT == 8) { pack_var64<8>(*reinterpret_cast<VarT<8>*>(vb), hv, ctx->R); used = reinterpret_cast<VarT<8>*>(vb)->used_mask; }
+            else { pack_var64<16>(*reinterpret_cast<VarT<16>*>(vb), hv, ctx->R); used = reinterpret_cast<VarT<16>*>(vb)->used_mask; }
             if (!used) return fail(ctx, HQS_E_INVALID, "class %u variant %u: empty request (request.rs:191-194)", c, v);
-            if (sc.variants[v].weight == 0) return fail(ctx, HQS_E_INVALID, "class %u variant %u: zero weight", c, v);
-            *min_time = sc.variants[v].min_time_ms;
-            masks[0] = sc.variants[v].all_mask & ((1u << ctx->R) - 1);
-            masks[1] = used;
+            if (hv.weight == 0) return fail(ctx, HQS_E_INVALID, "class %u variant %u: zero weight", c, v);
         }
     }
     CU(cudaSetDevice(ctx->device));
@@ -880,34 +869,10 @@ int hqs_classes_set(hqs_ctx* ctx, uint32_t n_classes, const hqs_class* classes) 
         memcpy(cb, &sc.n_variants, 4);
         for (u32 v = 0; v < sc.n_variants; ++v) {
             unsigned char* vb = cb + 8 + (size_t)v * var_bytes32;
-            u32* amount = reinterpret_cast<u32*>(vb);
-            float* rcp = reinterpret_cast<float*>(vb + (size_t)RT * 4);
-            u64* min_time = reinterpret_cast<u64*>(vb + (size_t)RT * 12);
-            u32* masks = reinterpret_cast<u32*>(vb + (size_t)RT * 12 + 8);
-            unsigned char* shb = vb + (size_t)RT * 12 + 16;                 // VarT::shw, one byte per resource
-            u32 used = 0;
-            for (u32 r = 0; r < ctx->R; ++r) {
-                const bool all = (sc.variants[v].all_mask >> r) & 1;
-                const u64 amt = all ? 0 : sc.variants[v].amount[r] / gs[r];
-                if (amt > NARROW_LIMIT) narrow_ok = false;
-                amount[r] = (u32)amt;
-                if (amt && amt <= NARROW_LIMIT) {
-                    // division by the invariant amount (see fit_count): magic number and the two shifts
-                    u32 l = 0;
-                    while (l < 32 && ((u64)1 << l) < amt) ++l;
-                    const u64 mm = (((u64)1 << 32) * (((u64)1 << l) - amt)) / amt + 1;
-                    const u32 magic = (u32)mm;
-                    memcpy(&rcp[r], &magic, 4);
-                    shb[r] = (unsigned char)((l < 1 ? l : 1) | ((l > 0 ? l - 1 : 0) << 1));
-                } else {
-                    rcp[r] = 0.0f;
-                }
-                rcp[RT + r] = all ? 0.0f : (float)(double)sc.variants[v].amount[r];
-                if (all || sc.variants[v].amount[r]) used |= 1u << r;
-            }
-            *min_time = sc.variants[v].min_time_ms;
-            masks[0] = sc.variants[v].all_mask & ((1u << ctx->R) - 1);
-            masks[1] = used;
+            const bool ok = RT == 4 ? pack_var32<4>(*reinterpret_cast<VarT<4, u32>*>(vb), sc.variants[v], ctx->R, gs)
+                          : RT == 8 ? pack_var32<8>(*reinterpret_cast<VarT<8, u32>*>(vb), sc.variants[v], ctx->R, gs)
+                                    : pack_var32<16>(*reinterpret_cast<VarT<16, u32>*>(vb), sc.variants[v], ctx->R, gs);
+            narrow_ok &= ok;
         }
     }
     ctx->narrow_classes = narrow_ok;

@@ -108,8 +108,19 @@ typedef struct {
     uint32_t coarsened;         /* 1 if LIVE priority levels had to be merged to fit HQS_MAX_GROUPS: tasks of merged
                                    levels are then ordered by class and handle, not by priority — log it         */
     uint32_t narrow_amounts;    /* 1 if the last tick solved on gcd-scaled 32-bit amounts          */
-    uint32_t reserved;
+    uint32_t solver_path;       /* HQS_PATH_* bits: how the last tick (or query) solved            */
 } hqs_stats;
+
+/* hqs_stats.solver_path.  The first four bits name the first-fit loops that ran (several can, one after the other:
+ * packed levels are followed by the general loop, a minimum-utilisation restart runs the solve again). */
+#define HQS_PATH_WIDE 0x01u            /* wide loop: every worker of a pool of <= 512 is a lane               */
+#define HQS_PATH_LEAN 0x02u            /* one-warp lean loop (plain tick)                                     */
+#define HQS_PATH_LEAN_EXTRAS 0x04u     /* lean loop with reservation / proactive-filling bookkeeping          */
+#define HQS_PATH_GENERAL 0x08u         /* general loop (variants, `All`, blocked masks, time limits, packing) */
+#define HQS_PATH_PACKED 0x10u          /* at least one saturated priority level was packed                    */
+#define HQS_PATH_MU_RESTART 0x20u      /* the minimum-utilisation rule restarted the solve                    */
+#define HQS_PATH_CLASSES_GLOBAL 0x40u  /* the class table did not fit shared memory and was read from global  */
+#define HQS_PATH_REM_GLOBAL 0x80u      /* narrow remainders did not fit shared memory and live in global       */
 
 int hqs_abi_version(void);
 

@@ -131,6 +131,7 @@ int hqs_tick(hqs_ctx* ctx, uint32_t W, const hqs_worker* workers, const uint64_t
     *out_n = n;
     if (free_after) std::copy(fr.begin(), fr.end(), free_after);
     ctx->stats.n_assigned = n;
+    ctx->stats.solver_path = 0;                             // no device solve loop runs in the double
     ctx->stats.ticks++;
     return HQS_OK;
 }

@@ -31,8 +31,9 @@ def _random_workload(n, w, q, r, vmax, seed, n_prio=5, cap=(8, 64)):
                       rng.integers(0, n_prio, n).astype(np.int32))
 
 
-def _check_exact(wl, expect_narrow=None):
-    """Both amount widths of the solver (gcd-scaled 32-bit and plain 64-bit) against the sequential spec."""
+def _check_exact(wl, expect_narrow=None, path_bits=0):
+    """Both amount widths of the solver (gcd-scaled 32-bit and plain 64-bit) against the sequential spec; path_bits:
+    HQS_PATH_* bits both ticks must report."""
     out = None
     for flags in (0, 2):
         s = P.gpu_scheduler(wl, flags=flags)
@@ -43,6 +44,7 @@ def _check_exact(wl, expect_narrow=None):
         assert np.array_equal(m.assignments, exp)
         assert np.array_equal(m.free_after, exp_free)
         narrow = s.stats()["narrow_amounts"]
+        assert s.stats()["solver_path"] & path_bits == path_bits, (flags, hex(s.stats()["solver_path"]))
         if flags == 2:
             assert narrow == 0
         elif expect_narrow is not None:
@@ -53,7 +55,8 @@ def _check_exact(wl, expect_narrow=None):
 
 
 def test_maximum_workers_resources_variants():
-    m = _check_exact(_random_workload(30000, 1024, 12, 16, 8, seed=1))
+    from hyperqueue_b200 import _lib as L
+    m = _check_exact(_random_workload(30000, 1024, 12, 16, 8, seed=1), path_bits=L.HQS_PATH_GENERAL)
     assert m.n_assigned() > 1000
 
 
@@ -63,7 +66,8 @@ def test_eight_resources_path():
 
 def test_large_class_table_uses_global_class_path():
     # 1500 classes x 648 B > the shared-memory budget of the solver => ClassT read from global memory
-    m = _check_exact(_random_workload(40000, 64, 1500, 4, 1, seed=3, n_prio=2))
+    from hyperqueue_b200 import _lib as L
+    m = _check_exact(_random_workload(40000, 64, 1500, 4, 1, seed=3, n_prio=2), path_bits=L.HQS_PATH_CLASSES_GLOBAL)
     assert m.n_assigned() > 100
 
 

@@ -23,10 +23,12 @@ FR = P.FR
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "oracle_drains.json")
 
 
-def _tick_vs_model(wl, levels=None):
+def _tick_vs_model(wl, levels=None, stats=None):
     s = P.gpu_scheduler(wl)
     free_before = s.free.copy()
     m = s.run_scheduling()
+    if stats is not None:
+        stats.update(s.stats())
     ready = np.ones(wl.n_tasks, dtype=bool)
     exp, exp_free = G.model_tick(wl, ready, free_before, levels)
     res = P.judge_tick(wl, free_before, m.assignments, ready)
@@ -52,7 +54,16 @@ def test_wide_first_fit_pool_shapes(n, w, q, seed, scale):
     """Plain ticks on pools of up to 512 workers run the wide first-fit (every worker a lane, one warp per 32 workers): ragged
     last warp (33, 300), all 16 warps (512), every task assignable (scale 1024) and saturated pools (scale 1: pack first, then
     dead classes are skipped); 513 workers fall back to the one-warp loop.  Bit-exact against the specification."""
-    _tick_vs_model(P.make_independent(n, w, q, seed, free_scale=scale))
+    from hyperqueue_b200 import _lib as L
+    st = {}
+    _tick_vs_model(P.make_independent(n, w, q, seed, free_scale=scale), stats=st)
+    path = st["solver_path"]
+    if w <= 512:
+        assert path & L.HQS_PATH_WIDE and not path & (L.HQS_PATH_LEAN | L.HQS_PATH_LEAN_EXTRAS), hex(path)
+    else:
+        assert path & L.HQS_PATH_LEAN and not path & L.HQS_PATH_WIDE, hex(path)
+    if scale == 1:
+        assert path & L.HQS_PATH_PACKED, hex(path)
 
 
 def test_tick_variants_and_blocked():
