@@ -14,7 +14,8 @@
 //                            scan:  exclusive prefix of the chunk table over chunks, one warp per group column;
 //                            pack:  on request, one warp fills one worker (pack_body, the first saturated level);
 //                            emit:  stable rank of every ready task inside its group -> count segment ->
-//                                   (worker, variant), 8-byte assignment, READY -> DONE.
+//                                   (worker, variant), 8-byte assignment, READY -> DONE; the assignments of a chunk
+//                                   are staged in shared memory and written as one contiguous run per group.
 // Phases are ordered by acquire/release counters in global memory (TickSync); every wait has a time-out, so a
 // broken grid fails the tick instead of hanging the GPU.  A sharded tick (several GPUs) exchanges the per-group
 // counts by NVLink peer stores from the solver CTA between the histogram and the solve.
@@ -40,7 +41,17 @@ struct TickSync {
     u32 emit_done;    // worker CTAs that left the kernel's work loop
     u32 error;        // 2 = a wait timed out
     u32 pad[2];
+#ifdef HQS_TRACE
+    unsigned long long tr_emit[6];   // measuring build: %globaltimer maxima over the worker CTAs of the emit steps (TR_EMIT_*), CTAs with work
+#endif
 };
+#ifdef HQS_TRACE
+// emit steps of a worker CTA: command seen, group records + segments staged, chunk filter done, emit_finish done, emit_done counted
+constexpr int TR_EMIT_CMD = 0, TR_EMIT_STAGED = 1, TR_EMIT_FILTER = 2, TR_EMIT_FINISH = 3, TR_EMIT_DONE = 4, TR_EMIT_NWORK = 5;
+#define TR_EMIT(a, i) { if (threadIdx.x == 0) atomicMax(&(a).sync->tr_emit[i], global_timer_ns()); }
+#else
+#define TR_EMIT(a, i)
+#endif
 
 // offsets into the solver CTA's dynamic shared memory (SM_NONE: the array stays in global memory)
 struct TickSmem {
@@ -68,6 +79,7 @@ struct TickArgs {
     // task table / chunk geometry
     u32* key;
     u32 n_handles, chunk, rows, P, nbits, emit_warps, g_smem;
+    u32 emit_stage;          // the finishing pass writes each chunk's assignments as per-group runs staged in shared memory
     // counts
     u32* total_local;        // [G] ready tasks of this rank per group (count step; zeroed at the end of the tick)
     const u32* total_ext;    // [G] counts summed over ranks, provided by the host (NCCL variant) or nullptr
@@ -186,7 +198,32 @@ __device__ void count_chunk(const TickArgs& a, u32 b, u32* s_hist) {
 // runs it WHILE the solver CTA solves and keeps its rows in registers; emit_finish needs the solver's group records.
 struct EmitRows { u32 kk[EMIT_ROWS_MAX], peers[EMIT_ROWS_MAX]; };
 
-__device__ __forceinline__ void emit_prepare(const TickArgs& a, u32 b, u32* s_cnt, EmitRows& er) {
+// the emit step's shared memory (worker CTAs)
+struct EmitSmem {
+    u32* cnt;              // [emit_warps][G] per-warp group counters
+    GroupOut* go;          // [G] the solver's group records (g_smem)
+    u32 *segc, *segw;      // [EMIT_SEG_SMEM] count segment cache
+    uint4* run;            // [G + 1] per-group runs of the chunk (emit_stage)
+    u32* slot;             // [chunk] staged tasks in run order (emit_stage)
+    unsigned short* q;     // [chunk] place of each task in its run (emit_stage)
+};
+
+__device__ __forceinline__ EmitSmem emit_smem(const TickArgs& a, unsigned char* smem) {
+    EmitSmem es;
+    es.cnt = reinterpret_cast<u32*>(smem);
+    es.go = reinterpret_cast<GroupOut*>(es.cnt + a.emit_warps * a.G);
+    es.segc = reinterpret_cast<u32*>(es.go + (a.g_smem ? a.G : 0));
+    es.segw = es.segc + EMIT_SEG_SMEM;
+    es.run = reinterpret_cast<uint4*>(reinterpret_cast<uintptr_t>(es.segw + EMIT_SEG_SMEM + 3) & ~(uintptr_t)15);   // 16-byte aligned
+    es.slot = reinterpret_cast<u32*>(es.run + a.G + 1);
+    es.q = reinterpret_cast<unsigned short*>(es.slot + a.chunk);
+    return es;
+}
+
+__device__ __forceinline__ void emit_stage_ranks(const TickArgs& a, u32 b, const EmitSmem& es, const EmitRows& er);
+
+__device__ __forceinline__ void emit_prepare(const TickArgs& a, u32 b, const EmitSmem& es, EmitRows& er) {
+    u32* s_cnt = es.cnt;
     const u32 G = a.G, Q = a.Q, nwarps = a.emit_warps, rows = a.rows;
     const u32 lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const u32* row = a.table + (size_t)b * G;
@@ -220,14 +257,17 @@ __device__ __forceinline__ void emit_prepare(const TickArgs& a, u32 b, u32* s_cn
     __syncthreads();
     // turn counts into starting ranks: rank0(w, g) = table[b][g] + sum_{w' < w} cnt[w'][g]
     for (u32 g = threadIdx.x; g < G; g += blockDim.x) {
-        u32 run = __ldcg(row + g);
+        const u32 first = __ldcg(row + g);
+        u32 run = first;
         for (u32 w2 = 0; w2 < nwarps; ++w2) {
             const u32 c = s_cnt[w2 * G + g];
             s_cnt[w2 * G + g] = run;
             run += c;
         }
+        if (a.emit_stage) es.run[g] = make_uint4(first, run - first, 0, 0);
     }
     __syncthreads();
+    if (a.emit_stage) emit_stage_ranks(a, b, es, er);
 }
 
 // A chunk holds an assigned task only if, for some group, fewer than k[g] tasks of the group precede the chunk (the
@@ -335,6 +375,142 @@ __device__ __forceinline__ void emit_finish(const TickArgs& a, u32 b, u32* s_cnt
     __syncthreads();
 }
 
+// Finishing pass on per-group runs (a.emit_stage).  The ready tasks of group g in chunk b have the consecutive local ranks
+// table[b][g] ... table[b][g] + cnt_b[g] - 1, and the assigned ones are the first n_b[g] of them, so the chunk's records form
+// ONE contiguous run of the output per group, starting at out_off[g] + table[b][g].  emit_stage_ranks (part of emit_prepare,
+// i.e. while the solver CTA still solves) writes every ready task to a shared-memory slot at its run's base + its place in
+// the run (bases: exclusive prefix of cnt_b over the groups) and remembers that place per task.  Once the group records
+// are out, emit_finish_staged writes the keys back row by row and flushes the slots in order, a thread per slot, so a warp
+// stores 32 consecutive records of a run instead of ~30 scattered ones.  A tick with a prefill range (kind-1 records
+// behind the assigned ranks) takes the per-task pass (emit_finish) on the same prepared rows.
+// Slot word: task offset inside the chunk (15 bits) | prefilled << 15 | group << 16.
+constexpr u32 STAGE_OFF_MASK = 0x7FFFu, STAGE_PF = 1u << 15, STAGE_G_SHIFT = 16;
+static_assert(TICK_THREADS * EMIT_ROWS_MAX <= STAGE_OFF_MASK + 1 && 2 * HQS_MAX_GROUPS <= (1u << (32 - STAGE_G_SHIFT)), "slot word");
+
+__device__ __forceinline__ void emit_stage_ranks(const TickArgs& a, u32 b, const EmitSmem& es, const EmitRows& er) {
+    __shared__ u32 s_wsum[TICK_WARPS];
+    const u32 G = a.G, Q = a.Q, nwarps = a.emit_warps, rows = a.rows;
+    const u32 lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const u32 base = b * a.chunk;
+    // es.run[g] = {table[b][g], cnt_b[g], slot base} (emit_prepare wrote the first two); a thread owns `per` consecutive
+    // groups, the slot bases are a block-wide exclusive prefix; es.run[G].x = ready tasks of the chunk
+    const u32 per = (G + blockDim.x - 1) / blockDim.x, g0 = min(threadIdx.x * per, G), g1 = min(g0 + per, G);
+    u32 sum = 0;
+    for (u32 g = g0; g < g1; ++g) { const u32 c = es.run[g].y; es.run[g].z = sum; sum += c; }
+    u32 inc = sum;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+        const u32 y = __shfl_up_sync(0xffffffffu, inc, d);
+        if ((int)lane >= d) inc += y;
+    }
+    if (lane == 31) s_wsum[warp] = inc;
+    __syncthreads();
+    u32 wbase = 0, n_ready = 0;
+    for (u32 w2 = 0; w2 < TICK_WARPS; ++w2) { const u32 v = s_wsum[w2]; wbase += w2 < warp ? v : 0u; n_ready += v; }
+    const u32 tbase = wbase + inc - sum;
+    for (u32 g = g0; g < g1; ++g) es.run[g].z += tbase;
+    if (threadIdx.x == 0) es.run[G] = make_uint4(n_ready, 0, 0, 0);
+    __syncthreads();
+    // ranks: the per-warp counters of emit_prepare, rows in order
+    const bool active = warp < nwarps;
+    const u32 wbeg = base + warp * (32 * rows);
+    u32* mycnt = es.cnt + (active ? warp : 0) * G;
+#pragma unroll
+    for (int j = 0; j < (int)EMIT_ROWS_MAX; ++j) {
+        if (active && j < (int)rows) {                       // warp-uniform
+            const u32 k = er.kk[j], pm = er.peers[j];
+            const u32 g = ((key_level(k) * Q + key_class(k)) << a.pf_shift) | ((k >> 28) & a.pf_shift);
+            if (pm) {
+                const u32 leader = __ffs(pm) - 1;
+                u32 r0 = 0;
+                if (leader == lane) {
+                    r0 = mycnt[g];
+                    mycnt[g] = r0 + __popc(pm);
+                }
+                r0 = __shfl_sync(pm, r0, leader);
+                const uint4 run = es.run[g];
+                const u32 q = r0 + __popc(pm & ((1u << lane) - 1)) - run.x;      // place in the chunk's run of the group
+                const u32 off = wbeg + j * 32 + lane - base;
+                es.slot[run.z + q] = off | ((k & KEY_PF) ? STAGE_PF : 0u) | (g << STAGE_G_SHIFT);
+                es.q[off] = (unsigned short)q;
+            }
+            __syncwarp();
+        }
+    }
+    __syncthreads();
+    // the counters back to the warps' starting ranks (the per-task pass reads them): warp w's counter now holds warp w+1's
+    for (u32 g = threadIdx.x; g < G; g += blockDim.x) {
+        for (u32 w2 = nwarps - 1; w2 > 0; --w2) es.cnt[w2 * G + g] = es.cnt[(w2 - 1) * G + g];
+        es.cnt[g] = es.run[g].x;
+    }
+    __syncthreads();
+}
+
+__device__ __forceinline__ void emit_finish_staged(const TickArgs& a, u32 b, const EmitSmem& es, bool seg_smem, const u32* before,
+                                                   const EmitRows& er) {
+    const u32 G = a.G, Q = a.Q, nwarps = a.emit_warps, rows = a.rows;
+    const u32 warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const u32 base = b * a.chunk;
+    const u32 n_ready = es.run[G].x;
+    // runs: es.run[g].y = assigned tasks (the first k[g] - before[g] - table[b][g] ranks, clamped to the run), .w = output
+    // index of the run's first record
+    for (u32 g = threadIdx.x; g < G; g += blockDim.x) {
+        const uint4 run = es.run[g];
+        const u32 bef = before ? __ldcg(before + g) : 0u;
+        const GroupOut go = es.go[g];
+        const u32 n = go.k > bef + run.x ? go.k - bef - run.x : 0u;
+        es.run[g].y = n < run.y ? n : run.y;
+        es.run[g].w = go.out_off + run.x;
+    }
+    __syncthreads();
+    // keys, row by row (coalesced): Waiting / Prefilled -> Assigned / Retracting
+    const bool active = warp < nwarps;
+    const u32 wbeg = base + warp * (32 * rows);
+#pragma unroll
+    for (int j = 0; j < (int)EMIT_ROWS_MAX; ++j) {
+        if (active && j < (int)rows && er.peers[j]) {
+            const u32 k = er.kk[j];
+            const u32 g = ((key_level(k) * Q + key_class(k)) << a.pf_shift) | ((k >> 28) & a.pf_shift);
+            const u32 i = wbeg + j * 32 + lane;
+            const u32 q = es.q[i - base];
+            const uint4 run = es.run[g];
+            if (q < run.y && run.w + q < a.out_cap) a.key[i] = (k & ~(KEY_READY | KEY_PF)) | KEY_DONE;
+        }
+    }
+    // flush: slot s is record run.w + (s - run.z) of its group's run when s - run.z < run.y
+    for (u32 s = threadIdx.x; s < n_ready; s += blockDim.x) {
+        const u32 v = es.slot[s];
+        const u32 g = v >> STAGE_G_SHIFT;
+        const uint4 run = es.run[g];
+        const u32 q = s - run.z;
+        if (q >= run.y) continue;
+        const u32 oi = run.w + q;
+        if (oi >= a.out_cap) continue;
+        const u32 r = run.x + q + (before ? __ldcg(before + g) : 0u);       // global rank in the group
+        const GroupOut go = es.go[g];
+        // first segment whose inclusive end rank exceeds r
+        u32 lo = go.seg_lo, hi = go.seg_lo + go.seg_n;
+        u32 wv;
+        if (seg_smem) {
+            while (lo < hi) {
+                const u32 mid = (lo + hi) >> 1;
+                if (es.segc[mid] > r) hi = mid; else lo = mid + 1;
+            }
+            wv = es.segw[lo];
+        } else {
+            while (lo < hi) {
+                const u32 mid = (lo + hi) >> 1;
+                if (__ldcg(a.seg_cum + mid) > r) hi = mid; else lo = mid + 1;
+            }
+            wv = __ldcg(a.seg_wv + lo);
+        }
+        // one 8-byte store: task | worker << 32 | variant << 48 | kind << 56 (hqs_assignment)
+        const u32 hi_word = (wv & 0xFFFFu) | (((wv >> 16) & 0xFFu) << 16) | ((v & STAGE_PF) ? 2u << 24 : 0u);
+        reinterpret_cast<uint2*>(a.out)[oi] = make_uint2(base + (v & STAGE_OFF_MASK), hi_word);
+    }
+    __syncthreads();
+}
+
 template <int RT>
 __device__ void worker_cta(const TickArgs& a, unsigned char* smem) {
     __shared__ u32 s_cmd, s_ok;
@@ -386,7 +562,7 @@ __device__ void worker_cta(const TickArgs& a, unsigned char* smem) {
         __syncthreads();
         prepared = s_ok != 0;
         __syncthreads();
-        if (prepared) emit_prepare(a, me, s_u32, er);
+        if (prepared) emit_prepare(a, me, emit_smem(a, smem), er);
     }
     // ---- command loop
     auto next_cmd = [&](u32 seen) -> u32 {
@@ -410,14 +586,13 @@ __device__ void worker_cta(const TickArgs& a, unsigned char* smem) {
     };
     // emit of this CTA's chunks; rows != nullptr: chunk `me` was prepared above
     auto do_emit = [&](EmitRows* rows) {
+        TR_EMIT(a, TR_EMIT_CMD)
         if (threadIdx.x == 0) s_ok = spin_until_ge(&a.sync->scan_done, nW) ? 1u : 0u;
         __syncthreads();
         if (s_ok) {
             const u32 G = a.G;
-            u32* s_cnt = s_u32;                                                      // [emit_warps][G]
-            GroupOut* s_go = reinterpret_cast<GroupOut*>(s_u32 + a.emit_warps * G);    // [G] when g_smem
-            u32* s_segc = reinterpret_cast<u32*>(s_go + (a.g_smem ? G : 0));          // [EMIT_SEG_SMEM]
-            u32* s_segw = s_segc + EMIT_SEG_SMEM;
+            const EmitSmem es = emit_smem(a, smem);
+            GroupOut* s_go = es.go;                                                  // [G] when g_smem
             const u32 n_seg = __ldcg(&a.hdr->n_segments);
             const bool seg_smem = n_seg <= EMIT_SEG_SMEM;
             const u32* before = a.x_world ? a.x_before : a.before_ext;
@@ -429,20 +604,35 @@ __device__ void worker_cta(const TickArgs& a, unsigned char* smem) {
                         s_go[g] = go;
                     }
                 if (seg_smem)
-                    for (u32 i = threadIdx.x; i < n_seg; i += blockDim.x) { s_segc[i] = __ldcg(a.seg_cum + i); s_segw[i] = __ldcg(a.seg_wv + i); }
+                    for (u32 i = threadIdx.x; i < n_seg; i += blockDim.x) { es.segc[i] = __ldcg(a.seg_cum + i); es.segw[i] = __ldcg(a.seg_wv + i); }
                 __syncthreads();
+                TR_EMIT(a, TR_EMIT_STAGED)
                 const u32 n_assigned = __ldcg(&a.hdr->n_assigned);
+                // kind-1 records of a prefill range lie behind the assigned ranks: such a tick keeps the per-task pass
+                const bool staged = a.emit_stage && __ldcg(&a.hdr->n_prefilled) == 0;
+                auto finish = [&](u32 b, const EmitRows& r) {
+                    if (staged) emit_finish_staged(a, b, es, seg_smem, before, r);
+                    else emit_finish(a, b, es.cnt, s_go, es.segc, es.segw, seg_smem, before, n_assigned, r);
+                };
                 if (rows) {
-                    if (emit_chunk_has_work(a, me, s_go, before))
-                        emit_finish(a, me, s_cnt, s_go, s_segc, s_segw, seg_smem, before, n_assigned, *rows);
+                    const bool work = emit_chunk_has_work(a, me, s_go, before);
+                    TR_EMIT(a, TR_EMIT_FILTER)
+                    if (work) {
+#ifdef HQS_TRACE
+                        if (threadIdx.x == 0) atomicAdd(&a.sync->tr_emit[TR_EMIT_NWORK], 1ull);
+#endif
+                        finish(me, *rows);
+                    }
                 } else {
                     for (u32 b = me; b < a.P; b += nW) {
                         if (!emit_chunk_has_work(a, b, s_go, before)) continue;
                         EmitRows r2;
-                        emit_prepare(a, b, s_cnt, r2);
-                        emit_finish(a, b, s_cnt, s_go, s_segc, s_segw, seg_smem, before, n_assigned, r2);
+                        emit_prepare(a, b, es, r2);
+                        finish(b, r2);
                     }
+                    TR_EMIT(a, TR_EMIT_FILTER)
                 }
+                TR_EMIT(a, TR_EMIT_FINISH)
             }
         } else if (threadIdx.x == 0) {
             atomicExch(&a.sync->error, 2u);
@@ -472,6 +662,7 @@ __device__ void worker_cta(const TickArgs& a, unsigned char* smem) {
     __syncthreads();
     if (threadIdx.x == 0) {
         __threadfence();
+        TR_EMIT(a, TR_EMIT_DONE)
         atomicAdd(&a.sync->emit_done, 1u);
     }
 }
@@ -495,6 +686,7 @@ __device__ void solver_cta(const TickArgs& a, unsigned char* smem) {
     __shared__ unsigned long long s_wx[2][TICK_WARPS];   // wide first-fit: one record per warp and group (double-buffered)
 #ifdef HQS_TRACE
     __shared__ u32 s_trw[8];
+    __shared__ unsigned long long s_trel;                // %globaltimer at the release of the grid's last command
 #endif
     __shared__ u32 s_wc[TICK_WARPS];                     //                 per warp: count segments written for the LAST group
     const u32 tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -1809,6 +2001,7 @@ __device__ void solver_cta(const TickArgs& a, unsigned char* smem) {
         // ---- release the worker CTAs as early as possible: they need the group records, the segments and n_segments
         u32 err = s_err ? 2u : (seg_overflow ? 1u : 0u);
         if (!err && n_assigned + n_prefilled > a.out_cap && (a.flags & TF_EMIT)) err = 3u;
+        if (err == 0 && (a.flags & TF_EMIT) && a.emit_stage && n_prefilled == 0) path |= HQS_PATH_EMIT_STAGED;     // as do_emit decides
         if (lane == 0) {
             a.hdr->n_segments = n_segments;
             a.hdr->n_assigned = n_assigned;
@@ -1817,6 +2010,9 @@ __device__ void solver_cta(const TickArgs& a, unsigned char* smem) {
             s_npref = n_prefilled;
             __threadfence();
             const u32 seq = s_npacks + 1;
+#ifdef HQS_TRACE
+            s_trel = global_timer_ns();
+#endif
             st_release(&a.sync->cmd, (seq << 2) | ((err == 0 && (a.flags & TF_EMIT)) ? CMD_EMIT : CMD_EXIT));
             s_final_err = err;
         }
@@ -1835,11 +2031,18 @@ __device__ void solver_cta(const TickArgs& a, unsigned char* smem) {
                 if (a.hdr_host) reinterpret_cast<u64*>(a.hdr_host + 1)[(size_t)w * R + r] = x;
             }
     }
+#ifdef HQS_TRACE
+    __syncthreads();
+    const unsigned long long tr_fv = global_timer_ns();     // free vectors written (device copy and pinned host mirror)
+#endif
     if (tid == 0) {
         if (!spin_until_ge(&a.sync->emit_done, nW)) s_err = 24;
     }
     __syncthreads();
     const long long t_end = clock64();
+#ifdef HQS_TRACE
+    const unsigned long long tr_seen = global_timer_ns();   // the solver CTA saw every worker CTA's emit_done
+#endif
     for (u32 g = tid; g < G; g += blockDim.x) a.total_local[g] = 0;
     if (tid == 0) {
         u32 err = s_final_err;
@@ -1869,9 +2072,21 @@ __device__ void solver_cta(const TickArgs& a, unsigned char* smem) {
         h.dbg[1] = ((unsigned long long)tr_fit << 32) | tr_load;
         for (int q = 0; q < 4; ++q) h.dbg[2 + q] = ((unsigned long long)tr_n[q] << 32) | tr_cyc[q];
         h.dbg[6] = (unsigned long long)(t_solved - t_prologue);
+        // emit tail, 16-bit fields in units of 16 ns after the release of the grid's last command (tools/trace_emit.py):
+        // dbg[7] = worker CTAs (maxima): command seen | staged | chunk filter | emit_finish;
+        // dbg[5] (wide loop) = emit_done counted | solver CTA: free vectors written | every emit_done seen | worker CTAs with work
+        auto d16 = [&](unsigned long long t) -> unsigned long long {
+            const unsigned long long d = t > s_trel ? (t - s_trel) >> 4 : 0;
+            return d < 0xFFFFu ? d : 0xFFFFu;
+        };
+        unsigned long long te[6];
+        for (int q = 0; q < 6; ++q) { te[q] = __ldcg(&a.sync->tr_emit[q]); a.sync->tr_emit[q] = 0; }
+        h.dbg[7] = d16(te[TR_EMIT_CMD]) | (d16(te[TR_EMIT_STAGED]) << 16) | (d16(te[TR_EMIT_FILTER]) << 32) | (d16(te[TR_EMIT_FINISH]) << 48);
         if (n_fast && tr_n[0] + tr_n[1] + tr_n[2] + tr_n[3] == 0) {      // the wide loop ran: its section sums (warp 0)
             for (int q = 0; q < 4; ++q) h.dbg[q] = ((unsigned long long)s_trw[2 * q + 1] << 32) | s_trw[2 * q];
             h.dbg[4] = n_visits;
+            h.dbg[5] = d16(te[TR_EMIT_DONE]) | (d16(tr_fv) << 16) | (d16(tr_seen) << 32) |
+                       ((te[TR_EMIT_NWORK] < 0xFFFFu ? te[TR_EMIT_NWORK] : 0xFFFFu) << 48);
         }
 #endif
         *a.hdr = h;

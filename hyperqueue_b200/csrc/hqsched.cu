@@ -444,7 +444,7 @@ void tick_orders(const hqs_ctx* ctx, u32 W, const u64* free_rw, const u64* total
 // Chunk geometry of the streaming steps: every worker CTA of the tick kernel owns chunks b, b + nW, ...; an emit warp owns
 // `rows` rows of 32 consecutive tasks of its chunk.  rows is chosen so that the table splits into (about) one chunk per
 // worker CTA; large tables take several chunks per CTA.
-struct TickGeom { u32 G, L, P, chunk, rows, emit_warps, g_smem, nbits; size_t worker_smem; };
+struct TickGeom { u32 G, L, P, chunk, rows, emit_warps, g_smem, nbits, emit_stage; size_t worker_smem; };
 
 TickGeom tick_geom(const hqs_ctx* ctx) {
     TickGeom t;
@@ -452,20 +452,26 @@ TickGeom tick_geom(const hqs_ctx* ctx) {
     t.G = (t.L * std::max<u32>(ctx->Q, 1)) << (ctx->pf_max ? 1 : 0);      // proactive filling: waiting / prefilled sub-groups
     t.nbits = 1;
     while ((1u << t.nbits) < t.G) t.nbits++;
+    const u32 n = std::max<u32>(ctx->n_handles, 1);
+    const u32 nW = std::max<u32>(ctx->grid_ctas - 1, 1);
     // emit step shared memory: warps * G counters (+ G solver records) + the segment cache
     const size_t seg_cache = 2 * EMIT_SEG_SMEM * sizeof(u32);
     t.emit_warps = TICK_WARPS;
     while (t.emit_warps > 1 && (size_t)t.emit_warps * t.G * 4 > 128 * 1024) t.emit_warps /= 2;
-    t.g_smem = ((size_t)t.emit_warps * t.G * 4 + (size_t)t.G * sizeof(GroupOut) + seg_cache <= 192 * 1024) ? 1 : 0;
-    const size_t emit_smem = (size_t)t.emit_warps * t.G * 4 + (t.g_smem ? (size_t)t.G * sizeof(GroupOut) : 0) + seg_cache;
-    const size_t pack_smem = (size_t)TICK_WARPS * PACK_MAX_CAND * sizeof(double);
-    t.worker_smem = std::max(std::max(emit_smem, pack_smem), (size_t)t.G * 4);
-    const u32 n = std::max<u32>(ctx->n_handles, 1);
-    const u32 nW = std::max<u32>(ctx->grid_ctas - 1, 1);
     const u32 per_row = t.emit_warps * 32;
     t.rows = std::min<u32>(EMIT_ROWS_MAX, std::max<u32>(1, (u32)(((u64)n + (u64)nW * per_row - 1) / ((u64)nW * per_row))));
     t.chunk = per_row * t.rows;
     t.P = (n + t.chunk - 1) / t.chunk;
+    t.g_smem = ((size_t)t.emit_warps * t.G * 4 + (size_t)t.G * sizeof(GroupOut) + seg_cache <= 192 * 1024) ? 1 : 0;
+    size_t emit_smem = (size_t)t.emit_warps * t.G * 4 + (t.g_smem ? (size_t)t.G * sizeof(GroupOut) : 0) + seg_cache;
+    // staged finishing pass (EmitSmem): + a 16-byte run record per group (+ one), a 4-byte slot and a 2-byte run place per
+    // task of the chunk.  Read on every tick, so that a test can compare both passes in one process.
+    const bool no_stage = getenv("HQS_DEBUG_EMIT_PER_TASK") != nullptr;     // measuring / testing aid: the per-task pass
+    const size_t stage_smem = ((emit_smem + 15) & ~(size_t)15) + ((size_t)t.G + 1) * 16 + (size_t)t.chunk * 6;
+    t.emit_stage = (t.g_smem && !no_stage && stage_smem <= 192 * 1024) ? 1 : 0;
+    if (t.emit_stage) emit_smem = stage_smem;
+    const size_t pack_smem = (size_t)TICK_WARPS * PACK_MAX_CAND * sizeof(double);
+    t.worker_smem = std::max(std::max(emit_smem, pack_smem), (size_t)t.G * 4);
     return t;
 }
 
@@ -588,7 +594,7 @@ TickArgs base_args(hqs_ctx* ctx, const TickGeom& t, u32 W, const TickLayout& lay
     a.W = W; a.Q = ctx->Q; a.L = t.L; a.R = ctx->R; a.G = t.G;
     a.classes_bytes = ctx->Q * (narrow ? ctx->class_bytes32 : ctx->class_bytes);
     a.key = ctx->d_key; a.n_handles = ctx->n_handles; a.chunk = t.chunk; a.rows = t.rows; a.P = t.P; a.nbits = t.nbits;
-    a.emit_warps = t.emit_warps; a.g_smem = t.g_smem;
+    a.emit_warps = t.emit_warps; a.g_smem = t.g_smem; a.emit_stage = t.emit_stage;
     a.total_local = ctx->d_total;
     a.table = ctx->d_table;
     a.gout = ctx->d_gout;

@@ -121,6 +121,9 @@ typedef struct {
 #define HQS_PATH_MU_RESTART 0x20u      /* the minimum-utilisation rule restarted the solve                    */
 #define HQS_PATH_CLASSES_GLOBAL 0x40u  /* the class table did not fit shared memory and was read from global  */
 #define HQS_PATH_REM_GLOBAL 0x80u      /* narrow remainders did not fit shared memory and live in global       */
+#define HQS_PATH_EMIT_STAGED 0x100u    /* the tick emitted each chunk's assignments as per-group runs staged in shared
+                                          memory; clear on an emitting tick: one pass per task (large group counts,
+                                          ticks with a prefill range, HQS_DEBUG_EMIT_PER_TASK)                  */
 
 int hqs_abi_version(void);
 
