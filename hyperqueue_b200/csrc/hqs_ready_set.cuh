@@ -28,11 +28,12 @@ struct TickHeaderOut {
     u32 n_assigned;  // local assignments
     u32 n_groups;
     u32 n_segments;
-    u32 error;       // 1 = segment overflow, 2 = a grid wait timed out, 3 = out_cap too small (nothing was emitted)
-    u32 n_prefilled; // prefill records (kind 1) behind the assignments
+    u32 error;       // 1 = segment overflow, 2 = a grid wait timed out, 3 = out_cap too small (nothing was emitted),
+                     // 4 = sharded tick: a peer has another group count G (nothing was solved or emitted)
+    u32 n_prefilled; // prefill records (kind 1) behind the assignments (this rank's, in a sharded tick)
     u32 pad;         // detail of error 2: which wait timed out
     u32 solver_path; // HQS_PATH_* bits: which solve loops ran (hqs_stats.solver_path)
-    u32 pad2;
+    u32 pad2;        // detail of error 4: 1 << 31 | peer rank << 16 | the peer's G
     unsigned long long dbg[8];   // clock64 phase lengths of the solver CTA (hqs_debug_read)
 };
 

@@ -356,7 +356,7 @@ __device__ __forceinline__ void emit_finish(const TickArgs& a, u32 b, u32* s_cnt
                             const u32 mid = (lo + hi) >> 1;
                             if (__ldcg(a.pf_cum + mid) > r) hi = mid; else lo = mid + 1;
                         }
-                        const u32 oi = n_assigned + g2.y + (r - go.k);
+                        const u32 oi = n_assigned + g2.y + (r - max(go.k, bef));      // sharded: this rank's part of the range
                         if (oi < a.out_cap) {
                             hqs_assignment asg;
                             asg.task = i;
@@ -608,7 +608,8 @@ __device__ void worker_cta(const TickArgs& a, unsigned char* smem) {
                 __syncthreads();
                 TR_EMIT(a, TR_EMIT_STAGED)
                 const u32 n_assigned = __ldcg(&a.hdr->n_assigned);
-                // kind-1 records of a prefill range lie behind the assigned ranks: such a tick keeps the per-task pass
+                // kind-1 records of a prefill range lie behind the assigned ranks: such a tick keeps the per-task pass (in a
+                // sharded tick n_prefilled is this rank's, so a rank without prefill records may stage while its peers do not)
                 const bool staged = a.emit_stage && __ldcg(&a.hdr->n_prefilled) == 0;
                 auto finish = [&](u32 b, const EmitRows& r) {
                     if (staged) emit_finish_staged(a, b, es, seg_smem, before, r);
@@ -683,6 +684,7 @@ __device__ void solver_cta(const TickArgs& a, unsigned char* smem) {
     __shared__ u32 s_pkpos[PACK_MAX_CAND], s_pknseg[PACK_MAX_CAND], s_pkseglo[PACK_MAX_CAND], s_pkex[PACK_MAX_CAND], s_cbase[PACK_MAX_CAND + 1];
     __shared__ u32 s_blk[8];            // block command: type, li, lj, seg region base, phi (2 words), n_packs
     __shared__ u32 s_nlist, s_multi, s_err, s_final_err, s_npacks, s_partial, s_npref, s_bign;
+    __shared__ u32 s_xmis;              // sharded tick: 1 << 31 | peer << 16 | the peer's G if a peer's group count differs
     __shared__ unsigned long long s_wx[2][TICK_WARPS];   // wide first-fit: one record per warp and group (double-buffered)
 #ifdef HQS_TRACE
     __shared__ u32 s_trw[8];
@@ -761,7 +763,7 @@ __device__ void solver_cta(const TickArgs& a, unsigned char* smem) {
     };
 
     // ---- prologue A: staging (overlaps the histogram of the worker CTAs)
-    if (tid == 0) { s_nlist = 0; s_multi = 0; s_err = 0; s_final_err = 0; s_npacks = 0; s_partial = 0; s_npref = 0; s_bign = 0; }
+    if (tid == 0) { s_nlist = 0; s_multi = 0; s_err = 0; s_final_err = 0; s_npacks = 0; s_partial = 0; s_npref = 0; s_bign = 0; s_xmis = 0; }
     if (tid < HQS_MAX_RESOURCES) { s_totmax[tid] = 0; s_D[tid] = 0; s_C[tid] = 0; }
     if (a.sm.classes != SM_NONE) {
         const uint4* src = reinterpret_cast<const uint4*>(a.classes);
@@ -814,11 +816,15 @@ __device__ void solver_cta(const TickArgs& a, unsigned char* smem) {
     const u32* before = a.before_ext;
     if (a.x_world) {
         // block-strided peer stores of my count vector into every rank's exchange buffer (own included), a system
-        // fence, then one release flag per peer; afterwards acquire every rank's flag of THIS tick
+        // fence, then one release flag per peer; afterwards acquire every rank's flag of THIS tick.  Next to the flags every
+        // rank publishes its group count G: a rank with another G (e.g. proactive filling on one rank only) lays its vector
+        // out differently, and summing it would solve on garbage, so the tick fails before anything is emitted.  Only G is
+        // compared; ranks with equal G but another prefill reserve / max or level / class set are not detected.
         const u32 parity = a.x_seq & 1u;
         for (u32 r = 0; r < a.x_world; ++r) {
             u32* dst = a.x_peer[r] + ((size_t)parity * HQS_MAX_PEERS + a.x_rank) * HQS_MAX_GROUPS;
             for (u32 g = tid; g < G; g += blockDim.x) dst[g] = __ldcg(a.total_local + g);
+            if (tid == 0) a.x_peer[r][(size_t)2 * HQS_MAX_PEERS * HQS_MAX_GROUPS + (2 + parity) * HQS_MAX_PEERS + a.x_rank] = G;
         }
         __threadfence_system();
         __syncthreads();
@@ -829,12 +835,17 @@ __device__ void solver_cta(const TickArgs& a, unsigned char* smem) {
         if (tid < a.x_world) {
             const u32* myflags = a.x_peer[a.x_rank] + (size_t)2 * HQS_MAX_PEERS * HQS_MAX_GROUPS + (size_t)parity * HQS_MAX_PEERS;
             const long long t0 = clock64();
+            bool got = true;
             while (ld_acquire_sys(myflags + tid) != a.x_seq) {
-                if (clock64() - t0 > PEER_TIMEOUT_CYCLES) { s_err = 22 + (tid << 8); break; }       // peer `tid` never sent its counts
+                if (clock64() - t0 > PEER_TIMEOUT_CYCLES) { s_err = 22 + (tid << 8); got = false; break; }       // peer `tid` never sent its counts
                 __nanosleep(32);
             }
+            const u32 pg = got ? __ldcg(myflags + 2 * HQS_MAX_PEERS + tid) : G;          // the peer's G (after its flag)
+            if (pg != G) atomicCAS(&s_xmis, 0u, 0x80000000u | (tid << 16) | pg);
         }
         __syncthreads();
+        // on a mismatch the solve runs on an empty ready set and the tick ends with error 4
+        const bool xmis = s_xmis != 0;
         const u32* xc = a.x_peer[a.x_rank] + (size_t)parity * HQS_MAX_PEERS * HQS_MAX_GROUPS;
         for (u32 g = tid; g < G; g += blockDim.x) {
             u32 all = 0, bef = 0;
@@ -843,8 +854,8 @@ __device__ void solver_cta(const TickArgs& a, unsigned char* smem) {
                 all += v;
                 bef += r < a.x_rank ? v : 0u;
             }
-            a.x_all[g] = all;
-            a.x_before[g] = bef;
+            a.x_all[g] = xmis ? 0u : all;
+            a.x_before[g] = xmis ? 0u : bef;
         }
         __syncthreads();
         tot_all = a.x_all;
@@ -1197,7 +1208,21 @@ __device__ void solver_cta(const TickArgs& a, unsigned char* smem) {
                         a.pf_wk[pf_seg + i] = s_td[i];
                     }
                     if (tid == 0) a.gout2[s_glist[et].x] = make_uint4(k + n_el * ps, pf_out, pf_seg, n_el);
-                    pf_out += n_el * ps;
+                    // records of this rank: a sharded tick emits only the part of the range [k, k + n_el * ps) that falls
+                    // into its own ranks [bef, bef + loc) of the group, so the offsets behind the assignments are local
+                    // (the sharded inputs are re-derived from `a` here rather than captured from the solve's scope, which
+                    // would keep them live in registers through the plain tick's solve)
+                    u32 share = n_el * ps;
+                    const u32* bef_g = a.x_world ? a.x_before : a.before_ext;
+                    if (bef_g) {
+                        const u32 g = s_glist[et].x;
+                        const bool sm = a.sm.bef != SM_NONE;
+                        const u32 bef = sm ? reinterpret_cast<const u32*>(smem + a.sm.bef)[et] : __ldcg(bef_g + g);
+                        const u32 loc = sm ? reinterpret_cast<const u32*>(smem + a.sm.loc)[et] : __ldcg(a.total_local + g);
+                        const u32 lo = max(k, bef), hi = min(k + n_el * ps, bef + loc);
+                        share = hi > lo ? hi - lo : 0u;
+                    }
+                    pf_out += share;
                     pf_seg += n_el;
                     bar_named(2, TICK_THREADS);
                 }
@@ -1989,7 +2014,7 @@ __device__ void solver_cta(const TickArgs& a, unsigned char* smem) {
             block_work(BLK_RESTART);
         }
         u32 n_prefilled = 0;
-        if (a.pf_shift && a.pf_max && (a.flags & TF_EMIT) && !before) {
+        if (a.pf_shift && a.pf_max && (a.flags & TF_EMIT)) {
             if (lane == 0) s_blk[0] = BLK_PREFILL;
             __syncwarp();
             bar_named(1, TICK_THREADS);
@@ -1999,7 +2024,7 @@ __device__ void solver_cta(const TickArgs& a, unsigned char* smem) {
         if (lane == 0) s_blk[0] = BLK_END;
         __syncwarp();
         // ---- release the worker CTAs as early as possible: they need the group records, the segments and n_segments
-        u32 err = s_err ? 2u : (seg_overflow ? 1u : 0u);
+        u32 err = s_err ? 2u : s_xmis ? 4u : (seg_overflow ? 1u : 0u);
         if (!err && n_assigned + n_prefilled > a.out_cap && (a.flags & TF_EMIT)) err = 3u;
         if (err == 0 && (a.flags & TF_EMIT) && a.emit_stage && n_prefilled == 0) path |= HQS_PATH_EMIT_STAGED;     // as do_emit decides
         if (lane == 0) {
@@ -2056,7 +2081,7 @@ __device__ void solver_cta(const TickArgs& a, unsigned char* smem) {
         h.n_prefilled = s_npref;
         h.pad = s_err ? s_err : (werr ? 25u : 0u);       // which wait timed out (21 histogram, 22 | peer << 8, 23 pack, 24 emit, 25 a worker CTA)
         h.solver_path = path;
-        h.pad2 = 0;
+        h.pad2 = s_xmis;                                  // detail of error 4: which peer, and its G
         h.dbg[0] = (unsigned long long)(t_counted - t_start);     // staging + wait for the histogram
         h.dbg[1] = (unsigned long long)(t_prologue - t_counted);  // exchange + compaction + demand
         h.dbg[2] = (unsigned long long)(t_solved - t_prologue);   // the solver warp

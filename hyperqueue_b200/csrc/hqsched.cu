@@ -716,6 +716,10 @@ int wait_header(hqs_ctx* ctx, TickHeaderOut* hdr) {
                     (unsigned long long)hdr->dbg[0], (unsigned long long)hdr->dbg[1]);
     }
     if (hdr->error == 1) return fail(ctx, HQS_E_LIMIT, "count-segment overflow (> %u segments in one tick)", SEG_CAP);
+    if (hdr->error == 4)
+        return fail(ctx, HQS_E_STATE, "sharded tick: this rank has G=%u groups, rank %u has G=%u (the number of levels, the classes and "
+                    "the proactive-filling setting must agree on every rank); nothing was scheduled", ctx->last_G, (hdr->pad2 >> 16) & 0x7FFFu,
+                    hdr->pad2 & 0xFFFFu);
     return HQS_OK;
 }
 
@@ -1159,6 +1163,7 @@ int hqs_tick_fetch(hqs_ctx* ctx, uint32_t out_cap, hqs_assignment* out, uint32_t
     if (out_n) *out_n = 0;
     CU(cudaSetDevice(ctx->device));
     ctx->tick_pending = false;
+    ctx->prefilled_wc.clear(); ctx->prefilled_W = 0;             // the mirror is per tick, whether the tick succeeded or not
     TickHeaderOut hdr;
     int rc = wait_header(ctx, &hdr);
     if (rc) return rc;
@@ -1171,7 +1176,6 @@ int hqs_tick_fetch(hqs_ctx* ctx, uint32_t out_cap, hqs_assignment* out, uint32_t
         CU(cudaMemcpyAsync(out, ctx->d_out, (size_t)n_rec * sizeof(hqs_assignment), cudaMemcpyDeviceToHost, ctx->stream));
         CU(cudaStreamSynchronize(ctx->stream));
     }
-    ctx->prefilled_wc.clear(); ctx->prefilled_W = 0;             // the mirror is per tick
     if (out_n) *out_n = n_rec;
     return HQS_OK;
 }
@@ -1256,7 +1260,8 @@ int hqs_shard_solve_emit(hqs_ctx* ctx, const uint32_t* d_counts_all, const uint3
     const TickGeom t = tick_geom(ctx);
     int rc = ensure_tick_buffers(ctx, t.G, t.P, ctx->last_W, out_cap);
     if (rc) return rc;
-    const TickLayout lay = tick_layout(ctx->last_W, ctx->R, ctx->Q, ctx->last_blocked);
+    // the tick input hqs_shard_count uploaded, prefill mask included (h_small[11] says whether it has one)
+    const TickLayout lay = tick_layout(ctx->last_W, ctx->R, ctx->Q, ctx->last_blocked, ctx->h_small[11] != 0);
     if ((rc = launch_tick(ctx, t, ctx->last_W, lay, ctx->last_blocked, d_counts_all, d_ranks_before, out_cap, true, false))) return rc;
     ctx->tick_pending = true;
     ctx->stats.ticks++;
@@ -1272,13 +1277,15 @@ int hqs_tick_reserve(hqs_ctx* ctx, uint32_t n_workers, uint32_t out_cap, int wit
     if (t.G > HQS_MAX_GROUPS) return fail(ctx, HQS_E_LIMIT, "groups=%u > %u", t.G, HQS_MAX_GROUPS);
     int rc = ensure_tick_buffers(ctx, t.G, t.P, n_workers, out_cap);
     if (rc) return rc;
-    const TickLayout lay = tick_layout(n_workers, ctx->R, ctx->Q, with_blocked != 0);
+    const TickLayout lay = tick_layout(n_workers, ctx->R, ctx->Q, with_blocked != 0, ctx->pf_max != 0);   // + the prefill mask
     if ((rc = ensure_tickin(ctx, lay.bytes))) return rc;
     CU(cudaStreamSynchronize(ctx->stream));
     return HQS_OK;
 }
 
-static size_t xbuf_bytes() { return ((size_t)2 * HQS_MAX_PEERS * HQS_MAX_GROUPS + 2 * HQS_MAX_PEERS) * sizeof(u32); }
+// exchange buffer: count vectors [parity][rank][HQS_MAX_GROUPS], release flags [parity][rank], group counts G [parity][rank]
+// (checked by the solver CTA: every rank runs the same library build, so the layout agrees)
+static size_t xbuf_bytes() { return ((size_t)2 * HQS_MAX_PEERS * HQS_MAX_GROUPS + 4 * HQS_MAX_PEERS) * sizeof(u32); }
 
 int hqs_shard_xbuf(hqs_ctx* ctx, void** d_xbuf, uint8_t ipc_handle[HQS_IPC_HANDLE_BYTES]) {
     if (!ctx) return HQS_E_INVALID;

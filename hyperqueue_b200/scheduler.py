@@ -100,6 +100,32 @@ class WorkerTaskMapping:
         return out
 
 
+def apply_tick_records(s, a: np.ndarray) -> Optional[np.ndarray]:
+    """The host's bookkeeping after a tick, on the scheduler `s` whose task handles the records `a` carry (a GpuScheduler,
+    or the per-rank one of a sharded tick): where each assigned task runs, the redirects of kind-2 records and the new
+    prefills of kind-1 records.  Returns, for the kind-2 records in order, the index of the worker each was prefilled on
+    (None if there are none)."""
+    retract_from = None
+    if a.size:
+        asg = a[a["kind"] != 1]
+        s._task_worker[asg["task"]] = asg["worker"]
+        s._task_variant[asg["task"]] = asg["variant"]
+        red = a[a["kind"] == 2]
+        if red.size:
+            # a prefilled task was assigned: RetractTasks to the worker that holds it, redirect to the new one; the
+            # new worker's resources are already taken (mapping.rs:49-101)
+            old = s._pf_worker[red["task"]].copy()
+            retract_from = np.searchsorted(s.worker_ids, old)
+            for t, ow, nwk, v in zip(red["task"].tolist(), old.tolist(), red["worker"].tolist(), red["variant"].tolist()):
+                s.redirects[t] = (int(s.worker_ids[nwk]), int(v))
+                s._retracting_from[t] = int(ow)
+            s._pf_worker[red["task"]] = -1
+        pf = a[a["kind"] == 1]
+        if pf.size:
+            s._pf_worker[pf["task"]] = s.worker_ids[pf["worker"]]
+    return retract_from
+
+
 class GpuScheduler:
     def __init__(self, n_resources: int, device: int = 0, flags: int = 0) -> None:
         self._lib = L.load_library()
@@ -316,14 +342,7 @@ class GpuScheduler:
         free_after = np.zeros_like(free)
         n = C.c_uint32(0)
         if self._prefill[1] > 0:
-            # "worker w holds a prefilled task of class c" (Worker::prefilled_tasks), the host's view at tick start
-            held = np.nonzero(self._pf_worker >= 0)[0]
-            pfwc = np.zeros((nw, len(self._classes)), dtype=np.uint8)
-            if held.size:
-                widx = np.searchsorted(self.worker_ids, self._pf_worker[held])
-                ok = (widx < nw) & (self.worker_ids[np.minimum(widx, nw - 1)] == self._pf_worker[held])
-                pfwc[widx[ok], self._task_class[held[ok]]] = 1
-            self._check(self._lib.hqs_prefill_state(self._ctx, nw, L.ptr(np.ascontiguousarray(pfwc))))
+            self._check(self._lib.hqs_prefill_state(self._ctx, nw, L.ptr(self.prefill_mask())))
         self._check(self._lib.hqs_tick(self._ctx, nw, L.ptr(w), L.ptr(free), L.ptr(total),
                                        L.ptr(blocked) if blocked is not None else None, out_cap,
                                        L.ptr(self._out), C.byref(n), L.ptr(free_after)))
@@ -331,25 +350,20 @@ class GpuScheduler:
         # WorkerConfiguration::min_utilization (solver.rs:154-156, 479-518) is enforced inside the tick kernel: a worker
         # that would receive less than its minimum is taken out of the solve, which then starts over
         self.free = free_after
-        retract_from = None
-        if a.size:
-            asg = a[a["kind"] != 1]
-            self._task_worker[asg["task"]] = asg["worker"]
-            self._task_variant[asg["task"]] = asg["variant"]
-            red = a[a["kind"] == 2]
-            if red.size:
-                # a prefilled task was assigned: RetractTasks to the worker that holds it, redirect to the new one; the
-                # new worker's resources are already taken (mapping.rs:49-101)
-                old = self._pf_worker[red["task"]].copy()
-                retract_from = np.searchsorted(self.worker_ids, old)
-                for t, ow, nwk, v in zip(red["task"].tolist(), old.tolist(), red["worker"].tolist(), red["variant"].tolist()):
-                    self.redirects[t] = (int(self.worker_ids[nwk]), int(v))
-                    self._retracting_from[t] = int(ow)
-                self._pf_worker[red["task"]] = -1
-            pf = a[a["kind"] == 1]
-            if pf.size:
-                self._pf_worker[pf["task"]] = self.worker_ids[pf["worker"]]
+        retract_from = apply_tick_records(self, a)
         return WorkerTaskMapping(a, self.worker_ids.copy(), free_after, retract_from)
+
+    def prefill_mask(self) -> np.ndarray:
+        """"Worker w holds a prefilled task of class c" (Worker::prefilled_tasks) over this scheduler's tasks, the host's
+        view at tick start: uint8 [W][Q], the input of hqs_prefill_state."""
+        nw = self.worker_ids.shape[0]
+        held = np.nonzero(self._pf_worker >= 0)[0]
+        pfwc = np.zeros((nw, len(self._classes)), dtype=np.uint8)
+        if held.size:
+            widx = np.searchsorted(self.worker_ids, self._pf_worker[held])
+            ok = (widx < nw) & (self.worker_ids[np.minimum(widx, nw - 1)] == self._pf_worker[held])
+            pfwc[widx[ok], self._task_class[held[ok]]] = 1
+        return np.ascontiguousarray(pfwc)
 
     # proactive filling ------------------------------------------------------------------------------
     def set_prefill(self, reserve: int, max_per_worker: int) -> None:
@@ -363,15 +377,24 @@ class GpuScheduler:
     def on_task_running_prefilled(self, handle: int, variant: int) -> None:
         """The worker started one of its prefilled tasks by itself (reactor.rs:263-345, RunningPrefilled): the task leaves
         the ready set and takes the worker's resources."""
+        pos = self._start_prefilled(handle, variant)
+        self._take_resources(pos, int(self._task_class[handle]), variant)
+
+    def _start_prefilled(self, handle: int, variant: int) -> int:
+        """Bookkeeping of on_task_running_prefilled without the free vectors; returns the worker's index."""
         wid = int(self._pf_worker[handle])
         assert wid >= 0, "task is not prefilled"
         pos = int(np.searchsorted(self.worker_ids, wid))
         self._pf_worker[handle] = -1
         self._task_worker[handle] = pos
         self._task_variant[handle] = variant
-        am = self._amount_tab[self._task_class[handle], variant]
-        self.free[pos] = np.where(self._all_tab[self._task_class[handle], variant], 0, self.free[pos] - np.minimum(self.free[pos], am))
         self.remove_ready_tasks(np.array([handle], dtype=np.uint32))
+        return pos
+
+    def _take_resources(self, pos: int, rq_id: int, variant: int) -> None:
+        """A task of class rq_id started on worker index pos with the given variant: it takes the worker's resources."""
+        am = self._amount_tab[rq_id, variant]
+        self.free[pos] = np.where(self._all_tab[rq_id, variant], 0, self.free[pos] - np.minimum(self.free[pos], am))
 
     def on_retract_response(self, worker_id: int, handles) -> Dict[int, List[Tuple[int, int]]]:
         """on_retract_response (server/reactor.rs:452-498): the worker gave the listed tasks back.  A task with a redirect

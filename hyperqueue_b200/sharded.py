@@ -18,17 +18,22 @@ host collective in between — the counting step's vector goes to every peer by 
 mapped exchange buffers, hqs_shard_xbuf / hqs_ipc_open / hqs_shard_attach) followed by a release flag, and the
 solver kernel acquires all flags and sums the vectors itself (hqs_shard_tick_launch).  torch.distributed is then
 used once, at set-up, to pass the 64-byte IPC handles around.
+
+Proactive filling works in both forms.  Each rank keeps the prefill state of its own tasks; before the tick the ranks OR
+their "worker holds a prefilled task of the class" masks (reduce_prefill_mask), so every rank solves with the same global
+mask, computes the same prefill ranges and emits the prefill records of its own tasks.
 """
 from __future__ import annotations
 
 import ctypes as C
-from typing import Optional, Tuple
+from typing import Dict, List, Optional, Tuple
 
 import numpy as np
 import torch
 import torch.distributed as dist
 
 from . import _lib as L
+from .scheduler import WorkerTaskMapping, apply_tick_records
 
 
 def shard_exchange(counts_local: torch.Tensor, rank: int, world: int,
@@ -42,6 +47,20 @@ def shard_exchange(counts_local: torch.Tensor, rank: int, world: int,
     counts_all = g2.sum(0).to(torch.int32)
     before = g2[:rank].sum(0).to(torch.int32) if rank else torch.zeros_like(counts_local)
     return counts_all, before
+
+
+def reduce_prefill_mask(mask_local: np.ndarray, world: int, group: Optional[dist.ProcessGroup] = None,
+                        device: Optional[torch.device] = None) -> np.ndarray:
+    """Proactive filling in a sharded tick: "worker w holds a prefilled task of class c" must hold over the tasks of ALL
+    ranks, but each rank knows only its own prefilled tasks.  Returns the OR of the ranks' uint8 [W][Q] masks (one
+    all-reduce, on `device` for NCCL); every rank passes the result to hqs_prefill_state."""
+    m = np.ascontiguousarray(mask_local, dtype=np.uint8)
+    if world == 1:
+        return m
+    dev = device if device is not None and dist.get_backend(group) == "nccl" else torch.device("cpu")
+    t = torch.from_numpy(m.copy()).to(dev)
+    dist.all_reduce(t, op=dist.ReduceOp.MAX, group=group)
+    return np.ascontiguousarray(t.cpu().numpy())
 
 
 def gather_peer_handles(sched, rank: int, world: int, group: Optional[dist.ProcessGroup] = None):
@@ -102,6 +121,7 @@ class ShardedScheduler:
         self.device = device
         self._counts = torch.zeros(L.HQS_MAX_GROUPS, dtype=torch.int32, device=device)
         self.p2p = bool(p2p)
+        self.last_mapping: Optional[WorkerTaskMapping] = None
         if self.p2p:
             attach_peers(sched, rank, world, group)
 
@@ -116,49 +136,92 @@ class ShardedScheduler:
             self.s.add_ready_tasks((h[m] - self.lo).astype(np.uint32), np.asarray(rq_ids)[m], np.asarray(priorities)[m])
 
     def run_scheduling(self, now: float = 0.0, out_cap: Optional[int] = None):
+        """One sharded tick.  Returns (this rank's records with GLOBAL handles, free vectors after the tick): its assignments
+        (kind 0 / 2) in single-context order, then its prefill records (kind 1).  self.last_mapping holds the same records
+        as a WorkerTaskMapping (messages(), retracts of kind-2 records)."""
         s = self.s
         s._sync_classes()
         w = s._worker_structs(now)
         free = np.ascontiguousarray(s.free)
         total = np.ascontiguousarray(s.total)
         blocked = s._blocked_bytes()
+        if s._prefill[1] > 0:
+            # a host collective at tick start: the previous tick has been fetched, so no collective overlaps a tick in
+            # flight (DESIGN.md §6); every rank passes the same global mask
+            pfwc = reduce_prefill_mask(s.prefill_mask(), self.world, self.group, self.device)
+            s._check(s._lib.hqs_prefill_state(s._ctx, w.shape[0], L.ptr(pfwc)))
+        cap = out_cap or max(self.hi - self.lo, 1)
         if self.p2p:
-            cap = out_cap or max(self.hi - self.lo, 1)
             s._check(s._lib.hqs_shard_tick_launch(s._ctx, w.shape[0], L.ptr(w), L.ptr(free), L.ptr(total),
                                                   L.ptr(blocked) if blocked is not None else None, cap))
-            out = np.zeros(cap, dtype=L.assignment_dtype)
-            free_after = np.zeros_like(free)
-            n = C.c_uint32(0)
-            s._check(s._lib.hqs_tick_fetch(s._ctx, cap, L.ptr(out), C.byref(n), L.ptr(free_after)))
-            a = out[: n.value].copy()
-            self._record(a)
-            a["task"] += np.uint32(self.lo)
-            s.free = free_after
-            return a, free_after
-        ng = C.c_uint32(0)
-        s._check(s._lib.hqs_shard_count(s._ctx, w.shape[0], L.ptr(w), L.ptr(free), L.ptr(total),
-                                        L.ptr(blocked) if blocked is not None else None,
-                                        C.c_void_p(self._counts.data_ptr()), self._counts.numel(), C.byref(ng)))
-        counts_all, before = shard_exchange(self._counts, self.rank, self.world, self.group)
-        torch.cuda.synchronize(self.device)
-        cap = out_cap or max(self.hi - self.lo, 1)
-        s._check(s._lib.hqs_shard_solve_emit(s._ctx, C.c_void_p(counts_all.data_ptr()), C.c_void_p(before.data_ptr()), cap))
+        else:
+            ng = C.c_uint32(0)
+            s._check(s._lib.hqs_shard_count(s._ctx, w.shape[0], L.ptr(w), L.ptr(free), L.ptr(total),
+                                            L.ptr(blocked) if blocked is not None else None,
+                                            C.c_void_p(self._counts.data_ptr()), self._counts.numel(), C.byref(ng)))
+            counts_all, before = shard_exchange(self._counts, self.rank, self.world, self.group)
+            torch.cuda.synchronize(self.device)
+            s._check(s._lib.hqs_shard_solve_emit(s._ctx, C.c_void_p(counts_all.data_ptr()), C.c_void_p(before.data_ptr()), cap))
         out = np.zeros(cap, dtype=L.assignment_dtype)
         free_after = np.zeros_like(free)
         n = C.c_uint32(0)
         s._check(s._lib.hqs_tick_fetch(s._ctx, cap, L.ptr(out), C.byref(n), L.ptr(free_after)))
         a = out[: n.value].copy()
-        self._record(a)
+        retract_from = self._record(a)
         a["task"] += np.uint32(self.lo)
         s.free = free_after
+        self.last_mapping = WorkerTaskMapping(a, s.worker_ids.copy(), free_after, retract_from)
         return a, free_after
 
-    def _record(self, a_local) -> None:
+    def _record(self, a_local):
         """TaskRuntimeState::Assigned{worker_id, rv_id} of this rank's tasks (local handles), as GpuScheduler.run_scheduling
-        keeps it: needed to return the resources when the tasks finish."""
-        if a_local.size:
-            self.s._task_worker[a_local["task"]] = a_local["worker"]
-            self.s._task_variant[a_local["task"]] = a_local["variant"]
+        keeps it (needed to return the resources when the tasks finish), and the rank's redirects and prefills."""
+        return apply_tick_records(self.s, a_local)
+
+    def _mine(self, handles) -> np.ndarray:
+        """This rank's handles among GLOBAL `handles`, as local handles."""
+        h = np.asarray(handles, dtype=np.int64).reshape(-1)
+        return h[(h >= self.lo) & (h < self.hi)] - self.lo
+
+    # proactive filling: every rank is called with the same arguments; handles are GLOBAL ---------------------------
+    def set_prefill(self, reserve: int, max_per_worker: int) -> None:
+        """SchedulerConfig::proactive_filling_reserve / _max; the same on every rank."""
+        self.s.set_prefill(reserve, max_per_worker)
+
+    def prefilled_tasks(self, worker_id: int) -> np.ndarray:
+        """This rank's tasks prefilled on the worker (global handles)."""
+        return self.s.prefilled_tasks(worker_id) + self.lo
+
+    def on_task_running_prefilled(self, handle: int, variant: int) -> None:
+        """The worker started one of its prefilled tasks (RunningPrefilled).  Only the owner knows the worker and the class,
+        so the owner's (worker index, class) is summed over the ranks (one all-reduce of two integers), and every rank takes
+        the same resources from its replicated free vectors."""
+        s = self.s
+        mine = self._mine([handle])
+        key = np.zeros(2, dtype=np.int64)
+        if mine.size:
+            loc = int(mine[0])
+            key[:] = (s._start_prefilled(loc, variant) + 1, int(s._task_class[loc]) + 1)
+        if self.world > 1:
+            t = torch.from_numpy(key)
+            dev = self.device if dist.get_backend(self.group) == "nccl" else torch.device("cpu")
+            t = t.to(dev)
+            dist.all_reduce(t, group=self.group)
+            key = t.cpu().numpy()
+        assert key[0] > 0, "task is not prefilled on any rank"
+        s._take_resources(int(key[0]) - 1, int(key[1]) - 1, variant)
+
+    def on_retract_response(self, worker_id: int, handles) -> Dict[int, List[Tuple[int, int]]]:
+        """The worker gave the listed tasks back; the owner of a redirected task returns it as target worker id ->
+        [(global handle, variant)]."""
+        sent = self.s.on_retract_response(worker_id, self._mine(handles))
+        return {wid: [(t + self.lo, v) for t, v in lst] for wid, lst in sent.items()}
+
+    def dispose_prefill(self, rq_id: int) -> Dict[int, List[int]]:
+        """check_dispose_prefill on every rank: each rank retracts its own prefilled tasks of the class and returns them as
+        worker id -> [global handles]."""
+        ret = self.s.dispose_prefill(rq_id)
+        return {wid: [t + self.lo for t in lst] for wid, lst in ret.items()}
 
     def tasks_finished(self, handles) -> None:
         """task_finished for GLOBAL handles, called with the same list on every rank: every rank holds the replicated free

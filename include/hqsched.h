@@ -123,7 +123,8 @@ typedef struct {
 #define HQS_PATH_REM_GLOBAL 0x80u      /* narrow remainders did not fit shared memory and live in global       */
 #define HQS_PATH_EMIT_STAGED 0x100u    /* the tick emitted each chunk's assignments as per-group runs staged in shared
                                           memory; clear on an emitting tick: one pass per task (large group counts,
-                                          ticks with a prefill range, HQS_DEBUG_EMIT_PER_TASK)                  */
+                                          ticks with prefill records, HQS_DEBUG_EMIT_PER_TASK; in a sharded tick this
+                                          is the rank's own prefill records, so the bit can differ between ranks)  */
 
 int hqs_abi_version(void);
 
@@ -228,14 +229,21 @@ int hqs_tick_reserve(hqs_ctx* ctx, uint32_t n_workers, uint32_t out_cap, int wit
  *                      contexts of one process pass each other's pointers directly)
  *   hqs_shard_tick_launch = hqs_tick_launch for rank `rank` of `world`: count -> peer stores + release flag ->
  *                      solve (acquires all flags, sums the vectors; same deterministic solve on every rank) ->
- *                      emit of this rank's tasks.  Fetch with hqs_tick_fetch.  All ranks must tick in lockstep. */
+ *                      emit of this rank's tasks.  Fetch with hqs_tick_fetch.  All ranks must tick in lockstep.
+ * Every rank publishes its number G of (level, class) groups next to its flag.  If a peer's G differs (for example proactive
+ * filling on one rank and off on another), hqs_tick_fetch returns HQS_E_STATE on every rank, with a text naming both counts;
+ * nothing was solved or emitted and the ready sets are unchanged.  Only G is compared: ranks with the same G but different
+ * prefill reserve / max values, or different level or class sets with the same number of groups, are NOT detected and
+ * silently compute different results; keeping them identical is the caller's job. */
 #define HQS_IPC_HANDLE_BYTES 64
 int hqs_shard_xbuf(hqs_ctx* ctx, void** d_xbuf, uint8_t ipc_handle[HQS_IPC_HANDLE_BYTES]);
 int hqs_ipc_open(hqs_ctx* ctx, const uint8_t ipc_handle[HQS_IPC_HANDLE_BYTES], void** d_ptr);
 int hqs_shard_attach(hqs_ctx* ctx, uint32_t world, uint32_t rank, void* const* peer_xbufs);
 int hqs_shard_tick_launch(hqs_ctx* ctx, uint32_t n_workers, const hqs_worker* workers, const uint64_t* free_rw,
                           const uint64_t* total_rw, const uint8_t* blocked_wcv, uint32_t out_cap);
-/* Device pointer / length of the last tick's assignment buffer (for NCCL all-gather of results). */
+/* Device pointer / length of the last tick's assignment buffer (for NCCL all-gather of results).  *d_out_n counts the
+ * assignments (kind 0 / 2) only; with proactive filling on, the tick's prefill records (kind 1) follow them in d_out and
+ * hqs_tick_fetch's *out_n counts both. */
 int hqs_device_result(hqs_ctx* ctx, const hqs_assignment** d_out, const uint32_t** d_out_n);
 
 /* Proactive filling (scheduler/mapping.rs:156-230, SchedulerConfig::proactive_filling_reserve / _max, state.rs:14-21;
@@ -249,7 +257,11 @@ int hqs_device_result(hqs_ctx* ctx, const hqs_assignment** d_out, const uint32_t
  * (hqs_prefill_state, bytes [n_workers][n_classes], consumed by the next tick), removes a prefilled task that a worker
  * started with hqs_ready_remove, and calls hqs_prefill_dispose(class) where TaskQueue::check_dispose_prefill
  * (taskqueue.rs:146-152: a task of higher priority became ready) retracts the class's prefills.
- * Not available in sharded ticks. */
+ * Sharded ticks (hqs_shard_count + hqs_shard_solve_emit, hqs_shard_tick_launch): every rank is configured with the same
+ * hqs_prefill_config and is given the same GLOBAL mask before each tick (worker w holds a prefilled task of class c, over
+ * the tasks of all ranks: only the host knows it).  The solve is replicated, so every rank computes the same prefill
+ * ranges; each rank emits the kind-1 records of its own tasks, behind its own assignments and in single-context order, and
+ * marks only those tasks prefilled.  hqs_prefill_dispose(class) is called on every rank and clears the rank's own tasks. */
 int hqs_prefill_config(hqs_ctx* ctx, uint32_t reserve, uint32_t max_per_worker);
 int hqs_prefill_state(hqs_ctx* ctx, uint32_t n_workers, const uint8_t* prefilled_wc);
 int hqs_prefill_dispose(hqs_ctx* ctx, uint32_t class_id);
