@@ -25,7 +25,7 @@ ABI_SYMBOLS = [
     "hqs_shard_count", "hqs_shard_solve_emit", "hqs_device_result", "hqs_ready_rearm", "hqs_stream", "hqs_sync",
     "hqs_get_stats", "hqs_set_stream", "hqs_set_profile", "hqs_get_kernel_ms", "hqs_debug_read", "hqs_levels_add", "hqs_query",
     "hqs_shard_xbuf", "hqs_ipc_open", "hqs_shard_attach", "hqs_shard_tick_launch", "hqs_tick_reserve",
-    "hqs_prefill_config", "hqs_prefill_state", "hqs_prefill_dispose", "hqs_ready_push_range",
+    "hqs_prefill_config", "hqs_prefill_state", "hqs_prefill_dispose", "hqs_ready_push_range", "hqs_debug_keys",
 ]
 HQS_IPC_HANDLE_BYTES = 64
 
@@ -134,6 +134,7 @@ def load_library() -> C.CDLL:
     lib.hqs_set_profile.argtypes = [vp, C.c_int]
     lib.hqs_get_kernel_ms.argtypes = [vp, C.POINTER(C.c_float)]
     lib.hqs_debug_read.argtypes = [vp, C.POINTER(C.c_uint64)]
+    lib.hqs_debug_keys.argtypes = [vp, u32, u32p, C.POINTER(C.c_uint32)]
     lib.hqs_levels_add.argtypes = [vp, u32, u64p]
     lib.hqs_query.argtypes = [vp, u32, vp, u64p, u64p, u8p, C.POINTER(C.c_uint32), u32p, u64p]
     lib.hqs_prefill_config.argtypes = [vp, u32, u32]

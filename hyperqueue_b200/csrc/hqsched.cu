@@ -97,6 +97,9 @@ struct hqs_ctx {
     size_t levels_pruned_at = 0;    // size of the level set after the last pruning
     u64* d_levels = nullptr;
     u32 d_levels_cap = 0;
+    u64* d_prune_lv = nullptr;      // prune_levels scratch: the exact levels and their live flags
+    u32* d_prune_live = nullptr;
+    u32 prune_cap = 0;
     // task table
     u32 n_handles = 0, cap_handles = 0;
     u32* d_key = nullptr;
@@ -229,8 +232,9 @@ int upload_levels(hqs_ctx* ctx) {
     return HQS_OK;
 }
 
+// Re-keys every VALID task from the current table.  An empty table (nothing is registered) puts any VALID key at level 0.
 int relevel_all(hqs_ctx* ctx) {
-    if (!ctx->n_handles || ctx->dev_levels.empty()) return HQS_OK;
+    if (!ctx->n_handles) return HQS_OK;
     relevel_k<<<(ctx->n_handles + 255) / 256, 256, 0, ctx->stream>>>(
         ctx->n_handles, ctx->d_key, ctx->d_prio, ctx->d_levels, (u32)ctx->dev_levels.size(), ctx->coarse ? 1 : 0);
     ctx->stats.kernel_launches++;
@@ -246,10 +250,18 @@ int prune_levels(hqs_ctx* ctx, bool* changed) {
     *changed = false;
     const u32 L = (u32)ctx->levels.size();
     if (ctx->levels_declared || L == 0 || ctx->n_handles == 0) return HQS_OK;
-    u64* d_lv = nullptr;
-    u32* d_live = nullptr;
-    CU(cudaMalloc(&d_lv, (size_t)L * 8));
-    CU(cudaMalloc(&d_live, (size_t)L * 4));
+    // scratch kept across calls: a coarse table is pruned on every push that brings a new priority, and cudaFree would
+    // synchronise the device each time
+    if (L > ctx->prune_cap) {
+        CU(cudaStreamSynchronize(ctx->stream));
+        if (ctx->d_prune_lv) { CU(cudaFree(ctx->d_prune_lv)); CU(cudaFree(ctx->d_prune_live)); }
+        ctx->d_prune_lv = nullptr; ctx->d_prune_live = nullptr;
+        ctx->prune_cap = std::max<u32>(L * 2, 4096);
+        CU(cudaMalloc(&ctx->d_prune_lv, (size_t)ctx->prune_cap * 8));
+        CU(cudaMalloc(&ctx->d_prune_live, (size_t)ctx->prune_cap * 4));
+    }
+    u64* d_lv = ctx->d_prune_lv;
+    u32* d_live = ctx->d_prune_live;
     CU(cudaMemsetAsync(d_live, 0, (size_t)L * 4, ctx->stream));
     CU(cudaMemcpyAsync(d_lv, ctx->levels.data(), (size_t)L * 8, cudaMemcpyHostToDevice, ctx->stream));
     level_live_k<<<(ctx->n_handles + 255) / 256, 256, 0, ctx->stream>>>(ctx->n_handles, ctx->d_key, ctx->d_prio, d_lv, L, d_live);
@@ -257,8 +269,6 @@ int prune_levels(hqs_ctx* ctx, bool* changed) {
     std::vector<u32> live(L);
     CU(cudaMemcpyAsync(live.data(), d_live, (size_t)L * 4, cudaMemcpyDeviceToHost, ctx->stream));
     CU(cudaStreamSynchronize(ctx->stream));
-    CU(cudaFree(d_lv));
-    CU(cudaFree(d_live));
     std::vector<u64> kept;
     kept.reserve(L);
     for (u32 i = 0; i < L; ++i)
@@ -806,7 +816,7 @@ void hqs_destroy(hqs_ctx* ctx) {
                         ctx->d_cons, ctx->d_push_task, ctx->d_push_cls, ctx->d_push_prio, ctx->d_newcnt,
                         ctx->d_newprio, ctx->d_table, ctx->d_total, ctx->d_gout, ctx->d_rem_scratch, ctx->d_excl, ctx->d_gout2, ctx->d_pf_cum, ctx->d_pf_wk, ctx->d_seg_cum,
                         ctx->d_seg_wv, ctx->d_out, ctx->d_hdr, ctx->d_free_after, ctx->d_tickin, ctx->d_sync, ctx->d_pk_fr,
-                        ctx->d_pk_quota, ctx->d_pk_taken, ctx->d_pk_cand, ctx->d_pk_meta};
+                        ctx->d_pk_quota, ctx->d_pk_taken, ctx->d_pk_cand, ctx->d_pk_meta, ctx->d_prune_lv, ctx->d_prune_live};
     for (void* p : dev_ptrs) if (p) cudaFree(p);
     for (void* p : ctx->x_opened) cudaIpcCloseMemHandle(p);
     if (ctx->d_xbuf) cudaFree(ctx->d_xbuf);
@@ -951,20 +961,29 @@ int push_impl(hqs_ctx* ctx, u32 n, const u32* task, u32 first_handle, const u32*
     ctx->stats.kernel_launches += 2;
     CU(cudaGetLastError());
     CU(cudaMemcpyAsync(ctx->h_small, ctx->d_newcnt, 2 * sizeof(u32), cudaMemcpyDeviceToHost, ctx->stream));
+    // a coarse table has a bucket for every priority, so push_k reports none as fresh: the batch's priorities are
+    // collected here, while the kernels run, and registered like fresh ones (the level set keeps growing, gets pruned
+    // and leaves coarse mode once the live priorities fit again).  Exact-mode pushes do not take this pass.
+    std::vector<u64> fresh;
+    if (ctx->coarse) distinct_priorities(priority, n, fresh);
     CU(cudaStreamSynchronize(ctx->stream));
     if (ctx->h_small[1]) return fail(ctx, HQS_E_INVALID, "a class id of the batch is >= n_classes %u (nothing was pushed)", ctx->Q);
     ctx->n_handles = std::max(ctx->n_handles, max_h + 1);
     ctx->stats.n_handles = ctx->n_handles;
     const u32 newcnt = ctx->h_small[0];
-    if (newcnt) {
-        std::vector<u64> fresh;
+    bool grew = false;
+    if (ctx->coarse) {
+        grew = merge_levels(ctx, fresh);
+    } else if (newcnt) {
         if (newcnt <= NEWPRIO_CAP) {
             fresh.resize(newcnt);
             CU(cudaMemcpy(fresh.data(), ctx->d_newprio, newcnt * sizeof(u64), cudaMemcpyDeviceToHost));
         } else {
             distinct_priorities(priority, n, fresh);
         }
-        merge_levels(ctx, fresh);
+        grew = merge_levels(ctx, fresh);
+    }
+    if (grew) {
         if (levels_need_pruning(ctx)) {
             bool dropped = false;
             if ((rc = prune_levels(ctx, &dropped))) return rc;
@@ -1408,6 +1427,21 @@ int hqs_sync(hqs_ctx* ctx) {
 int hqs_debug_read(hqs_ctx* ctx, uint64_t out[8]) {
     if (!ctx || !out) return HQS_E_INVALID;
     for (int i = 0; i < 8; ++i) out[i] = ctx->dbg[i];
+    return HQS_OK;
+}
+
+int hqs_debug_keys(hqs_ctx* ctx, uint32_t cap, uint32_t* keys, uint32_t* n_handles) {
+    if (!ctx) return HQS_E_INVALID;
+    if (ctx->tick_pending) return fail(ctx, HQS_E_STATE, "the previous tick has not been fetched");
+    if (cap && !keys) return fail(ctx, HQS_E_INVALID, "null key array");
+    CU(cudaSetDevice(ctx->device));
+    CU(cudaStreamSynchronize(ctx->stream));
+    const u32 n = std::min(cap, ctx->n_handles);
+    if (n) {
+        CU(cudaMemcpyAsync(keys, ctx->d_key, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream));
+        CU(cudaStreamSynchronize(ctx->stream));
+    }
+    if (n_handles) *n_handles = ctx->n_handles;
     return HQS_OK;
 }
 

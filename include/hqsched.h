@@ -283,6 +283,10 @@ int hqs_get_kernel_ms(hqs_ctx* ctx, float out_ms[4]);
  * histogram, [1] exchange + compaction + demand, [2] the solver warp, [3] emit, [4] non-empty groups, [5] whole
  * kernel, [6] whole kernel in nanoseconds (globaltimer), [7] pack commands. */
 int hqs_debug_read(hqs_ctx* ctx, uint64_t out[8]);
+/* Debug / test aid: waits for the context stream and copies the first min(cap, n_handles) words of the device task table
+ * (key[h]: bit31 READY, bit30 DONE, bit29 VALID, bit28 PREFILLED, bits 14..27 the priority level, bits 0..13 the class)
+ * into keys; *n_handles (optional) receives the table size.  HQS_E_STATE while a tick has not been fetched. */
+int hqs_debug_keys(hqs_ctx* ctx, uint32_t cap, uint32_t* keys, uint32_t* n_handles);
 int hqs_sync(hqs_ctx* ctx);
 int hqs_get_stats(hqs_ctx* ctx, hqs_stats* out);
 

@@ -242,7 +242,7 @@ def test_too_small_out_cap_fails_before_anything_is_consumed():
 def test_priority_levels_of_departed_tasks_are_pruned():
     """tako priorities carry a per-job component, so a long-running server sees ever new priority values.  Levels that no
     task of the table carries any more are dropped before the level set would have to be coarsened: after 6 waves of
-    1500 distinct priorities each (9000 values, far beyond HQS_MAX_GROUPS / 2 classes = 2048 levels) the ticks are still
+    1500 distinct priorities each (9000 values, far beyond HQS_MAX_GROUPS / 2 classes = 4096 levels) the ticks are still
     exact (priority order is kept), because at most one wave is alive at a time."""
     from hyperqueue_b200 import GpuScheduler, RequestVariant, priority_from_user
     s = GpuScheduler(1)
