@@ -26,6 +26,7 @@ ABI_SYMBOLS = [
     "hqs_get_stats", "hqs_set_stream", "hqs_set_profile", "hqs_get_kernel_ms", "hqs_debug_read", "hqs_levels_add", "hqs_query",
     "hqs_shard_xbuf", "hqs_ipc_open", "hqs_shard_attach", "hqs_shard_tick_launch", "hqs_tick_reserve",
     "hqs_prefill_config", "hqs_prefill_state", "hqs_prefill_dispose", "hqs_ready_push_range", "hqs_debug_keys",
+    "hqs_query_fetch", "hqs_shard_query_launch", "hqs_shard_query_solve",
 ]
 HQS_IPC_HANDLE_BYTES = 64
 
@@ -137,6 +138,9 @@ def load_library() -> C.CDLL:
     lib.hqs_debug_keys.argtypes = [vp, u32, u32p, C.POINTER(C.c_uint32)]
     lib.hqs_levels_add.argtypes = [vp, u32, u64p]
     lib.hqs_query.argtypes = [vp, u32, vp, u64p, u64p, u8p, C.POINTER(C.c_uint32), u32p, u64p]
+    lib.hqs_query_fetch.argtypes = [vp, C.POINTER(C.c_uint32), u32p, u64p]
+    lib.hqs_shard_query_launch.argtypes = [vp, u32, vp, u64p, u64p, u8p]
+    lib.hqs_shard_query_solve.argtypes = [vp, vp]
     lib.hqs_prefill_config.argtypes = [vp, u32, u32]
     lib.hqs_prefill_state.argtypes = [vp, u32, u8p]
     lib.hqs_prefill_dispose.argtypes = [vp, u32]

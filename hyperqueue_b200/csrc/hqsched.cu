@@ -140,10 +140,12 @@ struct hqs_ctx {
     unsigned char* h_hdr_dev = nullptr;
     size_t h_hdr_cap = 0;
     u32* h_small = nullptr;             // pinned scratch (counters)
+    u32* h_pw = nullptr;                // pinned [HQS_MAX_WORKERS]: per-worker task counts of the last query
     // last tick
     u32 last_W = 0, last_G = 0, last_L = 0;
     bool last_blocked = false;
-    bool tick_pending = false;
+    bool tick_pending = false;          // a tick or a query has been launched and not fetched
+    bool query_pending = false;         // ... and it is a query (hqs_query_fetch)
     bool own_stream = true;
     bool profile = false;
     bool pack = true;
@@ -733,6 +735,56 @@ int wait_header(hqs_ctx* ctx, TickHeaderOut* hdr) {
     return HQS_OK;
 }
 
+// What a query needs beyond a tick, set up by the first query or by hqs_tick_reserve (so ticks alone never pay for it): the
+// pinned per-worker counters and seg_worker_totals_k.  A page-locked allocation and a kernel's lazy load at its first launch
+// can synchronise the device, which would dead-lock a fused query waiting there for a peer context of this process: such
+// contexts reserve before their first query, as before their first tick.
+int ensure_query_buffers(hqs_ctx* ctx) {
+    if (ctx->h_pw) return HQS_OK;
+    cudaFuncAttributes fa;
+    CU(cudaFuncGetAttributes(&fa, (const void*)seg_worker_totals_k));
+    CU(cudaMallocHost(&ctx->h_pw, HQS_MAX_WORKERS * sizeof(u32)));
+    return HQS_OK;
+}
+
+// What-if query: the tick kernel without its emit step (nothing is emitted or consumed), then the per-worker task counts of
+// its count segments into the pinned buffer hqs_query_fetch reads.  Like a tick, the query is pending until it is fetched.
+// counts_all / exchange as for launch_tick (a query has no local share, so no ranks_before).
+int launch_query(hqs_ctx* ctx, const TickGeom& t, u32 W, const TickLayout& lay, bool blocked, const u32* d_counts_all,
+                 bool exchange) {
+    int rc = ensure_query_buffers(ctx);
+    if (rc) return rc;
+    rc = launch_tick(ctx, t, W, lay, blocked, d_counts_all, nullptr, 0, false, exchange);
+    if (rc) return rc;
+    u32* d_pw = ctx->d_pk_quota;    // scratch (pack is over): [W] counters
+    CU(cudaMemsetAsync(d_pw, 0, W * sizeof(u32), ctx->stream));
+    seg_worker_totals_k<<<(t.G + 127) / 128, 128, 0, ctx->stream>>>(ctx->d_gout, t.G, ctx->d_seg_cum, ctx->d_seg_wv, d_pw);
+    ctx->stats.kernel_launches++;
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(ctx->h_pw, d_pw, W * sizeof(u32), cudaMemcpyDeviceToHost, ctx->stream));
+    ctx->tick_pending = true;
+    ctx->query_pending = true;
+    return HQS_OK;
+}
+
+// shared body of hqs_query (exchange = false) and hqs_shard_query_launch: validation, tick input, launch
+int query_launch_impl(hqs_ctx* ctx, u32 n_workers, const hqs_worker* workers, const u64* free_rw, const u64* total_rw,
+                      const uint8_t* blocked_wcv, bool exchange) {
+    int rc = validate_workers(ctx, n_workers, workers, free_rw, total_rw);
+    if (rc) return rc;
+    if (ctx->tick_pending) return fail(ctx, HQS_E_STATE, "the previous tick has not been fetched");
+    CU(cudaSetDevice(ctx->device));
+    const TickGeom t = tick_geom(ctx);
+    if (t.G > HQS_MAX_GROUPS) return fail(ctx, HQS_E_LIMIT, "groups=%u > %u", t.G, HQS_MAX_GROUPS);
+    if ((rc = ensure_tick_buffers(ctx, t.G, t.P, n_workers, 1024))) return rc;
+    TickLayout lay;
+    bool has_mu, any_time;
+    if ((rc = upload_tick_input(ctx, n_workers, workers, free_rw, total_rw, blocked_wcv, &lay, &has_mu, &any_time))) return rc;
+    // ticks and queries share one exchange sequence: every rank advances it in lockstep
+    if (exchange) ctx->x_seq += 1;
+    return launch_query(ctx, t, n_workers, lay, blocked_wcv != nullptr, nullptr, exchange);
+}
+
 }  // namespace
 
 // ================================================================================================
@@ -825,6 +877,7 @@ void hqs_destroy(hqs_ctx* ctx) {
     if (ctx->h_tickin) cudaFreeHost(ctx->h_tickin);
     if (ctx->h_hdr) cudaFreeHost(ctx->h_hdr);
     if (ctx->h_small) cudaFreeHost(ctx->h_small);
+    if (ctx->h_pw) cudaFreeHost(ctx->h_pw);
     for (cudaEvent_t e : ctx->ev) if (e) cudaEventDestroy(e);
     if (ctx->stream && ctx->own_stream) cudaStreamDestroy(ctx->stream);
     delete ctx;
@@ -1179,6 +1232,7 @@ int hqs_tick_launch(hqs_ctx* ctx, uint32_t n_workers, const hqs_worker* workers,
 int hqs_tick_fetch(hqs_ctx* ctx, uint32_t out_cap, hqs_assignment* out, uint32_t* out_n, uint64_t* free_after) {
     if (!ctx) return HQS_E_INVALID;
     if (!ctx->tick_pending) return fail(ctx, HQS_E_STATE, "no tick in flight");
+    if (ctx->query_pending) return fail(ctx, HQS_E_STATE, "a query is in flight: fetch it with hqs_query_fetch");
     if (out_n) *out_n = 0;
     CU(cudaSetDevice(ctx->device));
     ctx->tick_pending = false;
@@ -1212,30 +1266,30 @@ int hqs_query(hqs_ctx* ctx, uint32_t n_workers, const hqs_worker* workers, const
               uint32_t* per_worker_assigned, uint64_t* free_after) {
     if (!ctx) return HQS_E_INVALID;
     if (n_would_assign) *n_would_assign = 0;
-    int rc = validate_workers(ctx, n_workers, workers, free_rw, total_rw);
+    const int rc = query_launch_impl(ctx, n_workers, workers, free_rw, total_rw, blocked_wcv, false);
     if (rc) return rc;
-    if (ctx->tick_pending) return fail(ctx, HQS_E_STATE, "the previous tick has not been fetched");
+    return hqs_query_fetch(ctx, n_would_assign, per_worker_assigned, free_after);
+}
+
+int hqs_query_fetch(hqs_ctx* ctx, uint32_t* n_would_assign, uint32_t* per_worker_assigned, uint64_t* free_after) {
+    if (!ctx) return HQS_E_INVALID;
+    if (n_would_assign) *n_would_assign = 0;
+    if (!ctx->tick_pending) return fail(ctx, HQS_E_STATE, "no query in flight");
+    if (!ctx->query_pending) return fail(ctx, HQS_E_STATE, "a tick is in flight: fetch it with hqs_tick_fetch");
     CU(cudaSetDevice(ctx->device));
-    const TickGeom t = tick_geom(ctx);
-    if (t.G > HQS_MAX_GROUPS) return fail(ctx, HQS_E_LIMIT, "groups=%u > %u", t.G, HQS_MAX_GROUPS);
-    if ((rc = ensure_tick_buffers(ctx, t.G, t.P, n_workers, 1024))) return rc;
-    TickLayout lay;
-    bool has_mu, any_time;
-    if ((rc = upload_tick_input(ctx, n_workers, workers, free_rw, total_rw, blocked_wcv, &lay, &has_mu, &any_time))) return rc;
-    // same kernel, no emit step: nothing is emitted or consumed
-    if ((rc = launch_tick(ctx, t, n_workers, lay, blocked_wcv != nullptr, nullptr, nullptr, 0, false, false))) return rc;
-    u32* d_pw = ctx->d_pk_quota;    // scratch (pack is over): [W] counters
-    CU(cudaMemsetAsync(d_pw, 0, n_workers * sizeof(u32), ctx->stream));
-    seg_worker_totals_k<<<(t.G + 127) / 128, 128, 0, ctx->stream>>>(ctx->d_gout, t.G, ctx->d_seg_cum, ctx->d_seg_wv, d_pw);
-    ctx->stats.kernel_launches++;
-    CU(cudaGetLastError());
-    std::vector<u32> pw(n_workers);
-    CU(cudaMemcpyAsync(pw.data(), d_pw, n_workers * sizeof(u32), cudaMemcpyDeviceToHost, ctx->stream));
+    ctx->tick_pending = false;
+    ctx->query_pending = false;
     TickHeaderOut hdr;
-    if ((rc = wait_header(ctx, &hdr))) return rc;
-    if (free_after) memcpy(free_after, ctx->h_hdr + sizeof(TickHeaderOut), (size_t)n_workers * ctx->R * 8);
-    if (n_would_assign) *n_would_assign = hdr.n_assigned;
-    if (per_worker_assigned) memcpy(per_worker_assigned, pw.data(), n_workers * sizeof(u32));
+    const int rc = wait_header(ctx, &hdr);
+    if (rc) return rc;
+    if (free_after) memcpy(free_after, ctx->h_hdr + sizeof(TickHeaderOut), (size_t)ctx->last_W * ctx->R * 8);
+    // the count segments cover every group's assigned ranks [0, k), so the per-worker counts sum to the tasks assigned over
+    // all ranks; the header's n_assigned of a sharded launch is this rank's share only (the solver's local output offsets)
+    u32 total = 0;
+    for (u32 w = 0; w < ctx->last_W; ++w) total += ctx->h_pw[w];
+    ctx->stats.n_assigned = total;
+    if (n_would_assign) *n_would_assign = total;
+    if (per_worker_assigned) memcpy(per_worker_assigned, ctx->h_pw, ctx->last_W * sizeof(u32));
     return HQS_OK;
 }
 
@@ -1298,6 +1352,7 @@ int hqs_tick_reserve(hqs_ctx* ctx, uint32_t n_workers, uint32_t out_cap, int wit
     if (rc) return rc;
     const TickLayout lay = tick_layout(n_workers, ctx->R, ctx->Q, with_blocked != 0, ctx->pf_max != 0);   // + the prefill mask
     if ((rc = ensure_tickin(ctx, lay.bytes))) return rc;
+    if ((rc = ensure_query_buffers(ctx))) return rc;
     CU(cudaStreamSynchronize(ctx->stream));
     return HQS_OK;
 }
@@ -1379,6 +1434,27 @@ int hqs_shard_tick_launch(hqs_ctx* ctx, uint32_t n_workers, const hqs_worker* wo
     ctx->tick_pending = true;
     ctx->stats.ticks++;
     return HQS_OK;
+}
+
+int hqs_shard_query_launch(hqs_ctx* ctx, uint32_t n_workers, const hqs_worker* workers, const uint64_t* free_rw,
+                           const uint64_t* total_rw, const uint8_t* blocked_wcv) {
+    if (!ctx) return HQS_E_INVALID;
+    if (!ctx->x_world) return fail(ctx, HQS_E_STATE, "hqs_shard_attach has not been called");
+    return query_launch_impl(ctx, n_workers, workers, free_rw, total_rw, blocked_wcv, true);
+}
+
+int hqs_shard_query_solve(hqs_ctx* ctx, const uint32_t* d_counts_all) {
+    if (!ctx) return HQS_E_INVALID;
+    if (!d_counts_all) return fail(ctx, HQS_E_INVALID, "null count vector");
+    if (!ctx->last_W) return fail(ctx, HQS_E_STATE, "hqs_shard_count has not been called");
+    if (ctx->tick_pending) return fail(ctx, HQS_E_STATE, "the previous tick has not been fetched");
+    CU(cudaSetDevice(ctx->device));
+    const TickGeom t = tick_geom(ctx);
+    int rc = ensure_tick_buffers(ctx, t.G, t.P, ctx->last_W, 1024);
+    if (rc) return rc;
+    // the tick input hqs_shard_count uploaded
+    const TickLayout lay = tick_layout(ctx->last_W, ctx->R, ctx->Q, ctx->last_blocked, ctx->h_small[11] != 0);
+    return launch_query(ctx, t, ctx->last_W, lay, ctx->last_blocked, d_counts_all, false);
 }
 
 int hqs_device_result(hqs_ctx* ctx, const hqs_assignment** d_out, const uint32_t** d_out_n) {

@@ -126,6 +126,26 @@ def apply_tick_records(s, a: np.ndarray) -> Optional[np.ndarray]:
     return retract_from
 
 
+def query_workers(worker_totals: np.ndarray, remaining_s: Optional[np.ndarray] = None,
+                  min_utilization: Optional[np.ndarray] = None) -> Tuple[np.ndarray, np.ndarray]:
+    """The fake-worker array of a what-if query (new_worker_query): worker ids 0..n-1, time limits in seconds (inf = none)
+    as milliseconds, min_utilization as given.  Returns (workers [L.worker_dtype], totals [W][R] u64); the totals are also
+    the free vectors."""
+    tot = np.ascontiguousarray(worker_totals, dtype=np.uint64)
+    nw = tot.shape[0]
+    w = np.zeros(nw, dtype=L.worker_dtype)
+    w["worker_id"] = np.arange(nw, dtype=np.uint32)
+    rem = np.full(nw, L.HQS_TIME_INF, dtype=np.uint64)
+    if remaining_s is not None:
+        r = np.asarray(remaining_s, dtype=np.float64)
+        finite = ~np.isinf(r)
+        rem[finite] = (np.maximum(r[finite], 0.0) * 1000.0).astype(np.uint64)
+    w["remaining_time_ms"] = rem
+    if min_utilization is not None:
+        w["min_utilization"] = np.asarray(min_utilization, dtype=np.float32)
+    return w, tot
+
+
 class GpuScheduler:
     def __init__(self, n_resources: int, device: int = 0, flags: int = 0) -> None:
         self._lib = L.load_library()
@@ -454,18 +474,8 @@ class GpuScheduler:
         resources (query.rs:35-46); remaining_s = time limits of the allocation (inf = none); min_utilization as in
         WorkerConfiguration.  Returns (needed[bool], counts, total)."""
         self._sync_classes()
-        tot = np.ascontiguousarray(worker_totals, dtype=np.uint64)
+        w, tot = query_workers(worker_totals, remaining_s, min_utilization)
         nw = tot.shape[0]
-        w = np.zeros(nw, dtype=L.worker_dtype)
-        w["worker_id"] = np.arange(nw, dtype=np.uint32)
-        rem = np.full(nw, L.HQS_TIME_INF, dtype=np.uint64)
-        if remaining_s is not None:
-            r = np.asarray(remaining_s, dtype=np.float64)
-            finite = ~np.isinf(r)
-            rem[finite] = (np.maximum(r[finite], 0.0) * 1000.0).astype(np.uint64)
-        w["remaining_time_ms"] = rem
-        if min_utilization is not None:
-            w["min_utilization"] = np.asarray(min_utilization, dtype=np.float32)
         counts = np.zeros(nw, dtype=np.uint32)
         n = C.c_uint32(0)
         self._check(self._lib.hqs_query(self._ctx, nw, L.ptr(w), L.ptr(tot), L.ptr(tot), None, C.byref(n), L.ptr(counts), None))

@@ -22,6 +22,10 @@ used once, at set-up, to pass the 64-byte IPC handles around.
 Proactive filling works in both forms.  Each rank keeps the prefill state of its own tasks; before the tick the ranks OR
 their "worker holds a prefilled task of the class" masks (reduce_prefill_mask), so every rank solves with the same global
 mask, computes the same prefill ranges and emits the prefill records of its own tasks.
+
+The autoalloc what-if query (ShardedScheduler.new_worker_query) runs the same two forms without the emit step
+(hqs_shard_query_launch, or hqs_shard_count + exchange + hqs_shard_query_solve): every rank solves the summed counts and
+returns the same answer, the one a single context holding all ranks' tasks gives.
 """
 from __future__ import annotations
 
@@ -33,7 +37,7 @@ import torch
 import torch.distributed as dist
 
 from . import _lib as L
-from .scheduler import WorkerTaskMapping, apply_tick_records
+from .scheduler import WorkerTaskMapping, apply_tick_records, query_workers
 
 
 def shard_exchange(counts_local: torch.Tensor, rank: int, world: int,
@@ -172,6 +176,32 @@ class ShardedScheduler:
         s.free = free_after
         self.last_mapping = WorkerTaskMapping(a, s.worker_ids.copy(), free_after, retract_from)
         return a, free_after
+
+    def new_worker_query(self, worker_totals: np.ndarray, now: float = 0.0, remaining_s: Optional[np.ndarray] = None,
+                         min_utilization: Optional[np.ndarray] = None):
+        """compute_new_worker_query (scheduler/query.rs:12-131) over the ready sets of ALL ranks: GpuScheduler.new_worker_query
+        on one context holding every rank's tasks, bit for bit.  Every rank calls it with the same arguments and gets the same
+        (needed[bool], counts, total); nothing is consumed.  It is an exchange like a tick: call it when no tick is in flight
+        (DESIGN.md §6).  `now` is accepted for symmetry with GpuScheduler: the fake workers' time limits are remaining_s."""
+        s = self.s
+        s._sync_classes()
+        w, tot = query_workers(worker_totals, remaining_s, min_utilization)
+        nw = tot.shape[0]
+        if self.p2p:
+            # no allocation between the launches of the ranks (contexts of one process wait for each other on the device)
+            s._check(s._lib.hqs_tick_reserve(s._ctx, nw, max(self.hi - self.lo, 1), 0))
+            s._check(s._lib.hqs_shard_query_launch(s._ctx, nw, L.ptr(w), L.ptr(tot), L.ptr(tot), None))
+        else:
+            ng = C.c_uint32(0)
+            s._check(s._lib.hqs_shard_count(s._ctx, nw, L.ptr(w), L.ptr(tot), L.ptr(tot), None,
+                                            C.c_void_p(self._counts.data_ptr()), self._counts.numel(), C.byref(ng)))
+            counts_all, _ = shard_exchange(self._counts, self.rank, self.world, self.group)
+            torch.cuda.synchronize(self.device)
+            s._check(s._lib.hqs_shard_query_solve(s._ctx, C.c_void_p(counts_all.data_ptr())))
+        counts = np.zeros(nw, dtype=np.uint32)
+        n = C.c_uint32(0)
+        s._check(s._lib.hqs_query_fetch(s._ctx, C.byref(n), L.ptr(counts), None))
+        return counts > 0, counts, int(n.value)
 
     def _record(self, a_local):
         """TaskRuntimeState::Assigned{worker_id, rv_id} of this rank's tasks (local handles), as GpuScheduler.run_scheduling

@@ -201,10 +201,18 @@ int hqs_tick_fetch(hqs_ctx* ctx, uint32_t out_cap, hqs_assignment* out, uint32_t
  * and the solver against an arbitrary (e.g. hypothetical, autoalloc) worker array WITHOUT emitting or consuming
  * anything: the ready set is unchanged.  per_worker_assigned[n_workers] (optional) receives how many tasks each
  * worker would get — a fake worker is "needed" iff its count is > 0; free_after as in hqs_tick.  Partial
- * descriptors use HQS_AMOUNT_MAX for unknown resources (query.rs:35-46). */
+ * descriptors use HQS_AMOUNT_MAX for unknown resources (query.rs:35-46).
+ * On a context of a sharded ready set (hqs_shard_attach) hqs_query answers for the tasks of THIS rank only; the answer over
+ * all ranks is hqs_shard_query_launch (or hqs_shard_count + hqs_shard_query_solve) on every rank, below. */
 int hqs_query(hqs_ctx* ctx, uint32_t n_workers, const hqs_worker* workers, const uint64_t* free_rw,
               const uint64_t* total_rw, const uint8_t* blocked_wcv, uint32_t* n_would_assign,
               uint32_t* per_worker_assigned, uint64_t* free_after);
+/* Fetches a query launched by hqs_shard_query_launch or hqs_shard_query_solve (hqs_query == launch + this fetch on one
+ * context): outputs as in hqs_query, with the launch's n_workers entries.  A query is pending like a tick until it is
+ * fetched: every call that fails with "the previous tick has not been fetched" fails the same way, hqs_tick_fetch on a
+ * pending query and hqs_query_fetch on a pending tick or with nothing pending return HQS_E_STATE and leave the pending launch
+ * fetchable.  A query does not count in hqs_stats.ticks. */
+int hqs_query_fetch(hqs_ctx* ctx, uint32_t* n_would_assign, uint32_t* per_worker_assigned, uint64_t* free_after);
 
 /* Multi-GPU sharding (SURVEY.md §8(e)): each rank owns a contiguous handle range of the task table.
  * Phase 1 counts the rank's ready tasks per group into d_counts (device pointer, n_groups_cap u32).
@@ -241,6 +249,22 @@ int hqs_ipc_open(hqs_ctx* ctx, const uint8_t ipc_handle[HQS_IPC_HANDLE_BYTES], v
 int hqs_shard_attach(hqs_ctx* ctx, uint32_t world, uint32_t rank, void* const* peer_xbufs);
 int hqs_shard_tick_launch(hqs_ctx* ctx, uint32_t n_workers, const hqs_worker* workers, const uint64_t* free_rw,
                           const uint64_t* total_rw, const uint8_t* blocked_wcv, uint32_t out_cap);
+
+/* What-if query over a sharded ready set.  Contract: every rank holds the same classes, declared levels, prefill
+ * configuration and fake-worker array; then every rank returns the same answer, and it is what hqs_query returns on ONE
+ * context holding the union of the ranks' ready sets (n_would_assign, per-worker counts, free vectors, bit for bit).  Nothing
+ * is emitted or consumed on any rank.  Fetch with hqs_query_fetch on every rank.
+ *   hqs_shard_query_launch  fused form, the counterpart of hqs_shard_tick_launch: one tick kernel with the peer exchange and
+ *                           without the emit step.  Ticks and queries share one exchange sequence, so all ranks must call it
+ *                           in lockstep, like a tick.  After hqs_tick_reserve with at least n_workers it allocates nothing
+ *                           (contexts of one process wait for each other on the device).  Ranks with different G fail it as a
+ *                           tick: hqs_query_fetch returns HQS_E_STATE on every rank, naming both counts; the ready sets are
+ *                           unchanged.
+ *   hqs_shard_query_solve   NCCL form: after hqs_shard_count (same worker array) with the all-gathered totals counts_all
+ *                           (device pointer, as for hqs_shard_solve_emit; a query emits nothing, so no ranks_before). */
+int hqs_shard_query_launch(hqs_ctx* ctx, uint32_t n_workers, const hqs_worker* workers, const uint64_t* free_rw,
+                           const uint64_t* total_rw, const uint8_t* blocked_wcv);
+int hqs_shard_query_solve(hqs_ctx* ctx, const uint32_t* d_counts_all);
 /* Device pointer / length of the last tick's assignment buffer (for NCCL all-gather of results).  *d_out_n counts the
  * assignments (kind 0 / 2) only; with proactive filling on, the tick's prefill records (kind 1) follow them in d_out and
  * hqs_tick_fetch's *out_n counts both. */
