@@ -6,8 +6,9 @@ entry point needs the compiled library and a CUDA device and fails loudly otherw
 """
 from ._lib import (HqsError, LibraryNotBuilt, assignment_dtype, load_library, HQS_AMOUNT_MAX, HQS_TIME_INF,
                    HQS_MAX_RESOURCES, HQS_MAX_VARIANTS, HQS_MAX_WORKERS, HQS_MAX_CLASSES, HQS_MAX_GROUPS)
-from .scheduler import (FRACTIONS_PER_UNIT, GpuScheduler, RequestVariant, WorkerTaskMapping, priority_from_user)
+from .scheduler import (FRACTIONS_PER_UNIT, GpuScheduler, GroupedTaskMapping, RequestVariant, WorkerTaskMapping,
+                        priority_from_user)
 
-__all__ = ["GpuScheduler", "RequestVariant", "WorkerTaskMapping", "HqsError", "LibraryNotBuilt", "load_library",
+__all__ = ["GpuScheduler", "RequestVariant", "WorkerTaskMapping", "GroupedTaskMapping", "HqsError", "LibraryNotBuilt", "load_library",
            "assignment_dtype", "priority_from_user", "FRACTIONS_PER_UNIT", "HQS_AMOUNT_MAX", "HQS_TIME_INF",
            "HQS_MAX_RESOURCES", "HQS_MAX_VARIANTS", "HQS_MAX_WORKERS", "HQS_MAX_CLASSES", "HQS_MAX_GROUPS"]

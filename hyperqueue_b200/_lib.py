@@ -27,6 +27,7 @@ ABI_SYMBOLS = [
     "hqs_shard_xbuf", "hqs_ipc_open", "hqs_shard_attach", "hqs_shard_tick_launch", "hqs_tick_reserve",
     "hqs_prefill_config", "hqs_prefill_state", "hqs_prefill_dispose", "hqs_ready_push_range", "hqs_debug_keys",
     "hqs_query_fetch", "hqs_shard_query_launch", "hqs_shard_query_solve",
+    "hqs_tick_fetch_grouped", "hqs_tick_grouped", "hqs_grouped_reserve", "hqs_grouped_kernel_ms",
 ]
 HQS_IPC_HANDLE_BYTES = 64
 
@@ -90,6 +91,11 @@ def load_shim() -> C.CDLL:
         _shim = C.CDLL(SHIM_PATH)
         _shim.hqshim_selftest.argtypes = [C.c_int, C.c_int]
         _shim.hqshim_selftest.restype = C.c_int
+        _shim.hqshim_selftest_grouped.argtypes = [C.c_int, C.c_int]
+        _shim.hqshim_selftest_grouped.restype = C.c_int
+        _shim.hqshim_time_mapping.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_int,
+                                              C.c_uint32, C.c_void_p, C.POINTER(C.c_uint64)]
+        _shim.hqshim_time_mapping.restype = C.c_int
     return _shim
 
 
@@ -118,6 +124,10 @@ def load_library() -> C.CDLL:
     lib.hqs_tick.argtypes = [vp, u32, vp, u64p, u64p, u8p, u32, vp, C.POINTER(C.c_uint32), u64p]
     lib.hqs_tick_launch.argtypes = [vp, u32, vp, u64p, u64p, u8p, u32]
     lib.hqs_tick_fetch.argtypes = [vp, u32, vp, C.POINTER(C.c_uint32), u64p]
+    lib.hqs_tick_fetch_grouped.argtypes = [vp, u32, vp, C.POINTER(C.c_uint32), u32, u32p, u64p]
+    lib.hqs_tick_grouped.argtypes = [vp, u32, vp, u64p, u64p, u8p, u32, vp, C.POINTER(C.c_uint32), u32, u32p, u64p]
+    lib.hqs_grouped_reserve.argtypes = [vp, u32, u32]
+    lib.hqs_grouped_kernel_ms.argtypes = [vp, C.POINTER(C.c_float)]
     lib.hqs_shard_count.argtypes = [vp, u32, vp, u64p, u64p, u8p, vp, u32, C.POINTER(C.c_uint32)]
     lib.hqs_shard_solve_emit.argtypes = [vp, vp, vp, u32]
     lib.hqs_tick_reserve.argtypes = [vp, u32, u32, C.c_int]

@@ -26,6 +26,8 @@
 // Sharded over several GPUs (one context per GPU, tasks block-sharded, workers replicated) the solver CTA stores the
 // rank's count vector into every peer's exchange buffer over NVLink and acquires the peers' flags before it solves (no
 // host collective).
+// hqs_tick_fetch_grouped regroups the tick's records per worker at fetch time (hqs_group.cuh: three plain launches behind
+// the tick; tick_k does not know about it).
 // The algorithm has a sequential specification, tests/greedy_model.py, which the kernels equal bit for bit.
 #include "../../include/hqsched.h"
 
@@ -52,6 +54,7 @@ typedef uint64_t u64;
 #include "hqs_ready_set.cuh"
 #include "hqs_solver.cuh"
 #include "hqs_tick.cuh"
+#include "hqs_group.cuh"
 
 
 // ================================================================================================
@@ -141,6 +144,13 @@ struct hqs_ctx {
     size_t h_hdr_cap = 0;
     u32* h_small = nullptr;             // pinned scratch (counters)
     u32* h_pw = nullptr;                // pinned [HQS_MAX_WORKERS]: per-worker task counts of the last query
+    // per-worker grouping of the records (hqs_tick_fetch_grouped); nothing of it exists until the first grouped fetch or
+    // hqs_grouped_reserve
+    hqs_assignment* d_grp_out = nullptr; u32 grp_cap = 0;      // the grouped records
+    u32* d_grp_hist = nullptr; size_t grp_hist_cap = 0;        // [2W + 1][tiles] counts, then their prefix over the tiles
+    u32* d_grp_small = nullptr;         // key totals [GRP_KEYS_MAX], offset table [GRP_KEYS_MAX + 1], the scan's ticket
+    u32* h_grp_off = nullptr;           // pinned mirror of the offset table
+    float grp_ms = -1.f;                // device time of the last grouping (profiling on), < 0: none
     // last tick
     u32 last_W = 0, last_G = 0, last_L = 0;
     bool last_blocked = false;
@@ -785,6 +795,93 @@ int query_launch_impl(hqs_ctx* ctx, u32 n_workers, const hqs_worker* workers, co
     return launch_query(ctx, t, n_workers, lay, blocked_wcv != nullptr, nullptr, exchange);
 }
 
+// Per-worker grouping (hqs_group.cuh).  Like the query's extras, its buffers and kernels are set up by the first grouped fetch
+// or by hqs_grouped_reserve, so a context that only fetches flat allocates and loads what it always did.
+constexpr u32 GRP_KEYS_MAX = 2 * HQS_MAX_WORKERS + 1;
+
+int ensure_group_buffers(hqs_ctx* ctx, u32 W, u32 cap) {
+    if (!ctx->d_grp_small) {
+        cudaFuncAttributes fa;
+        CU(cudaFuncGetAttributes(&fa, (const void*)group_count_k));
+        CU(cudaFuncGetAttributes(&fa, (const void*)group_scan_k));
+        CU(cudaFuncGetAttributes(&fa, (const void*)group_scatter_k));
+        CU(cudaFuncSetAttribute((const void*)group_scatter_k, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                (int)group_scatter_smem(HQS_MAX_WORKERS)));
+        CU(cudaMallocHost(&ctx->h_grp_off, (GRP_KEYS_MAX + 1) * sizeof(u32)));
+        CU(cudaMalloc(&ctx->d_grp_small, (2 * GRP_KEYS_MAX + 2) * sizeof(u32)));
+        CU(cudaMemsetAsync(ctx->d_grp_small, 0, (2 * GRP_KEYS_MAX + 2) * sizeof(u32), ctx->stream));   // the ticket starts at 0
+    }
+    if (cap > ctx->grp_cap) {
+        CU(cudaStreamSynchronize(ctx->stream));
+        if (ctx->d_grp_out) CU(cudaFree(ctx->d_grp_out));
+        ctx->d_grp_out = nullptr;
+        ctx->grp_cap = std::max<u32>(cap, 1024);
+        CU(cudaMalloc(&ctx->d_grp_out, (size_t)ctx->grp_cap * sizeof(hqs_assignment)));
+    }
+    const size_t need = (size_t)(2 * W + 1) * ((ctx->grp_cap + GROUP_TILE - 1) / GROUP_TILE);
+    if (need > ctx->grp_hist_cap) {
+        CU(cudaStreamSynchronize(ctx->stream));
+        if (ctx->d_grp_hist) CU(cudaFree(ctx->d_grp_hist));
+        ctx->d_grp_hist = nullptr;
+        ctx->grp_hist_cap = need;
+        CU(cudaMalloc(&ctx->d_grp_hist, need * sizeof(u32)));
+    }
+    return HQS_OK;
+}
+
+// d_out[0..n) -> d_grp_out grouped by worker, offset table behind the key totals in d_grp_small
+int launch_grouping(hqs_ctx* ctx, u32 n, u32 W) {
+    const u32 K = 2 * W + 1, T = (n + GROUP_TILE - 1) / GROUP_TILE;
+    u32* d_tot = ctx->d_grp_small;
+    u32* d_off = d_tot + GRP_KEYS_MAX;
+    u32* d_ticket = d_off + GRP_KEYS_MAX + 1;
+    const bool timed = ctx->profile && ctx->ev[1];
+    if (timed) CU(cudaEventRecord(ctx->ev[1], ctx->stream));
+    group_count_k<<<T, GROUP_THREADS, K * sizeof(u32), ctx->stream>>>(ctx->d_out, n, W, T, ctx->d_grp_hist);
+    group_scan_k<<<(K + GROUP_SCAN_THREADS / 32 - 1) / (GROUP_SCAN_THREADS / 32), GROUP_SCAN_THREADS, 0, ctx->stream>>>(
+        ctx->d_grp_hist, K, T, d_tot, d_off, d_ticket);
+    group_scatter_k<<<T, GROUP_THREADS, group_scatter_smem(W), ctx->stream>>>(ctx->d_out, n, W, T, ctx->d_grp_hist, d_off,
+                                                                            ctx->d_grp_out);
+    ctx->stats.kernel_launches += 3;
+    CU(cudaGetLastError());
+    if (timed) CU(cudaEventRecord(ctx->ev[2], ctx->stream));
+    return HQS_OK;
+}
+
+// shared body of hqs_tick_fetch (worker_off == nullptr) and hqs_tick_fetch_grouped
+int tick_fetch_impl(hqs_ctx* ctx, u32 out_cap, hqs_assignment* out, u32* out_n, u64* free_after, u32* worker_off) {
+    if (out_n) *out_n = 0;
+    CU(cudaSetDevice(ctx->device));
+    ctx->tick_pending = false;
+    ctx->prefilled_wc.clear(); ctx->prefilled_W = 0;             // the mirror is per tick, whether the tick succeeded or not
+    TickHeaderOut hdr;
+    int rc = wait_header(ctx, &hdr);
+    if (rc) return rc;
+    // error 3: the solver saw that out_cap is too small BEFORE the emit step: nothing was emitted, the ready set is intact
+    const u32 n_rec = hdr.n_assigned + hdr.n_prefilled;           // assignments (kind 0 / 2), then prefills (kind 1)
+    if (hdr.error == 3 || n_rec > out_cap || (n_rec && !out))
+        return fail(ctx, HQS_E_OVERFLOW, "out_cap=%u too small for %u assignments + %u prefills", out_cap, hdr.n_assigned, hdr.n_prefilled);
+    if (free_after) memcpy(free_after, ctx->h_hdr + sizeof(TickHeaderOut), (size_t)ctx->last_W * ctx->R * 8);
+    const u32 W = ctx->last_W, n_off = 2 * W + 2;
+    if (worker_off) memset(worker_off, 0, n_off * sizeof(u32));
+    if (n_rec && !worker_off) {
+        CU(cudaMemcpyAsync(out, ctx->d_out, (size_t)n_rec * sizeof(hqs_assignment), cudaMemcpyDeviceToHost, ctx->stream));
+        CU(cudaStreamSynchronize(ctx->stream));
+    } else if (n_rec) {
+        // n and the error word are known here, so the grids are exact and a failed tick never reaches this point
+        ctx->grp_ms = -1.f;
+        if ((rc = ensure_group_buffers(ctx, W, std::max(n_rec, ctx->out_cap_dev)))) return rc;
+        if ((rc = launch_grouping(ctx, n_rec, W))) return rc;
+        CU(cudaMemcpyAsync(out, ctx->d_grp_out, (size_t)n_rec * sizeof(hqs_assignment), cudaMemcpyDeviceToHost, ctx->stream));
+        CU(cudaMemcpyAsync(ctx->h_grp_off, ctx->d_grp_small + GRP_KEYS_MAX, n_off * sizeof(u32), cudaMemcpyDeviceToHost, ctx->stream));
+        CU(cudaStreamSynchronize(ctx->stream));
+        memcpy(worker_off, ctx->h_grp_off, n_off * sizeof(u32));
+        if (ctx->profile && ctx->ev[1] && cudaEventElapsedTime(&ctx->grp_ms, ctx->ev[1], ctx->ev[2]) != cudaSuccess) ctx->grp_ms = -1.f;
+    }
+    if (out_n) *out_n = n_rec;
+    return HQS_OK;
+}
+
 }  // namespace
 
 // ================================================================================================
@@ -878,6 +975,10 @@ void hqs_destroy(hqs_ctx* ctx) {
     if (ctx->h_hdr) cudaFreeHost(ctx->h_hdr);
     if (ctx->h_small) cudaFreeHost(ctx->h_small);
     if (ctx->h_pw) cudaFreeHost(ctx->h_pw);
+    if (ctx->d_grp_out) cudaFree(ctx->d_grp_out);
+    if (ctx->d_grp_hist) cudaFree(ctx->d_grp_hist);
+    if (ctx->d_grp_small) cudaFree(ctx->d_grp_small);
+    if (ctx->h_grp_off) cudaFreeHost(ctx->h_grp_off);
     for (cudaEvent_t e : ctx->ev) if (e) cudaEventDestroy(e);
     if (ctx->stream && ctx->own_stream) cudaStreamDestroy(ctx->stream);
     delete ctx;
@@ -1233,23 +1334,45 @@ int hqs_tick_fetch(hqs_ctx* ctx, uint32_t out_cap, hqs_assignment* out, uint32_t
     if (!ctx) return HQS_E_INVALID;
     if (!ctx->tick_pending) return fail(ctx, HQS_E_STATE, "no tick in flight");
     if (ctx->query_pending) return fail(ctx, HQS_E_STATE, "a query is in flight: fetch it with hqs_query_fetch");
-    if (out_n) *out_n = 0;
-    CU(cudaSetDevice(ctx->device));
-    ctx->tick_pending = false;
-    ctx->prefilled_wc.clear(); ctx->prefilled_W = 0;             // the mirror is per tick, whether the tick succeeded or not
-    TickHeaderOut hdr;
-    int rc = wait_header(ctx, &hdr);
+    return tick_fetch_impl(ctx, out_cap, out, out_n, free_after, nullptr);
+}
+
+int hqs_tick_fetch_grouped(hqs_ctx* ctx, uint32_t out_cap, hqs_assignment* out, uint32_t* out_n, uint32_t off_cap,
+                           uint32_t* worker_off, uint64_t* free_after) {
+    if (!ctx) return HQS_E_INVALID;
+    if (!ctx->tick_pending) return fail(ctx, HQS_E_STATE, "no tick in flight");
+    if (ctx->query_pending) return fail(ctx, HQS_E_STATE, "a query is in flight: fetch it with hqs_query_fetch");
+    // checked before the tick is consumed: it stays fetchable
+    if (!worker_off || off_cap < 2 * ctx->last_W + 2)
+        return fail(ctx, HQS_E_INVALID, "worker_off needs 2 * n_workers + 2 = %u entries (off_cap=%u)", 2 * ctx->last_W + 2, off_cap);
+    return tick_fetch_impl(ctx, out_cap, out, out_n, free_after, worker_off);
+}
+
+int hqs_tick_grouped(hqs_ctx* ctx, uint32_t n_workers, const hqs_worker* workers, const uint64_t* free_rw,
+                     const uint64_t* total_rw, const uint8_t* blocked_wcv, uint32_t out_cap, hqs_assignment* out,
+                     uint32_t* out_n, uint32_t off_cap, uint32_t* worker_off, uint64_t* free_after) {
+    if (!ctx) return HQS_E_INVALID;
+    if (!worker_off || (uint64_t)off_cap < 2 * (uint64_t)n_workers + 2)
+        return fail(ctx, HQS_E_INVALID, "worker_off needs 2 * n_workers + 2 entries (off_cap=%u)", off_cap);
+    int rc = hqs_tick_launch(ctx, n_workers, workers, free_rw, total_rw, blocked_wcv, out_cap);
     if (rc) return rc;
-    // error 3: the solver saw that out_cap is too small BEFORE the emit step: nothing was emitted, the ready set is intact
-    const u32 n_rec = hdr.n_assigned + hdr.n_prefilled;           // assignments (kind 0 / 2), then prefills (kind 1)
-    if (hdr.error == 3 || n_rec > out_cap || (n_rec && !out))
-        return fail(ctx, HQS_E_OVERFLOW, "out_cap=%u too small for %u assignments + %u prefills", out_cap, hdr.n_assigned, hdr.n_prefilled);
-    if (free_after) memcpy(free_after, ctx->h_hdr + sizeof(TickHeaderOut), (size_t)ctx->last_W * ctx->R * 8);
-    if (n_rec) {
-        CU(cudaMemcpyAsync(out, ctx->d_out, (size_t)n_rec * sizeof(hqs_assignment), cudaMemcpyDeviceToHost, ctx->stream));
-        CU(cudaStreamSynchronize(ctx->stream));
-    }
-    if (out_n) *out_n = n_rec;
+    return hqs_tick_fetch_grouped(ctx, out_cap, out, out_n, off_cap, worker_off, free_after);
+}
+
+int hqs_grouped_reserve(hqs_ctx* ctx, uint32_t n_workers, uint32_t out_cap) {
+    if (!ctx) return HQS_E_INVALID;
+    if (n_workers == 0 || n_workers > HQS_MAX_WORKERS) return fail(ctx, HQS_E_LIMIT, "n_workers=%u outside 1..%u", n_workers, HQS_MAX_WORKERS);
+    CU(cudaSetDevice(ctx->device));
+    int rc = ensure_group_buffers(ctx, n_workers, std::max(out_cap, ctx->out_cap_dev));
+    if (rc) return rc;
+    CU(cudaStreamSynchronize(ctx->stream));
+    return HQS_OK;
+}
+
+int hqs_grouped_kernel_ms(hqs_ctx* ctx, float* out_ms) {
+    if (!ctx || !out_ms) return HQS_E_INVALID;
+    if (ctx->grp_ms < 0) return fail(ctx, HQS_E_STATE, "no profiled grouped fetch available");
+    *out_ms = ctx->grp_ms;
     return HQS_OK;
 }
 

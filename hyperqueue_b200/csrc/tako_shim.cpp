@@ -179,22 +179,26 @@ hqs_stats GpuCore::stats() const {
     return st;
 }
 
-// run_scheduling_inner (main.rs:40-46): builds the per-tick worker view, runs the tick, applies the result to the
-// host mirror (Worker::insert_sn_task: free -= request; task state Waiting -> Assigned) and groups it per worker.
-WorkerTaskMapping GpuCore::run_scheduling(uint64_t now_ms) {
-    WorkerTaskMapping mapping;
+// The per-tick worker view of run_scheduling_inner (main.rs:40-46) in the form the C ABI takes: pending classes and ready
+// tasks are flushed, the workers come in ascending id, the record buffer is sized, the prefill mask is handed over.
+// Returns false when there is nothing to schedule.
+bool GpuCore::tick_input(uint64_t now_ms, TickInput& in) {
     flush_classes();
     flush_ready();
     const uint32_t W = (uint32_t)workers_.size();
-    if (W == 0 || classes_.empty() || tasks_.empty()) return mapping;
+    if (W == 0 || classes_.empty() || tasks_.empty()) return false;
     const uint32_t Q = (uint32_t)classes_.size();
-    std::vector<hqs_worker> hw(W);
-    std::vector<uint64_t> free_rw((size_t)W * R_), total_rw((size_t)W * R_), free_after((size_t)W * R_);
-    std::vector<uint8_t> blocked;
-    std::vector<WorkerId> ids(W);
+    std::vector<hqs_worker>& hw = in.hw;
+    std::vector<uint64_t>&free_rw = in.free_rw, &total_rw = in.total_rw;
+    std::vector<uint8_t>& blocked = in.blocked;
+    std::vector<WorkerId>& ids = in.ids;
+    hw.assign(W, hqs_worker{});
+    free_rw.assign((size_t)W * R_, 0); total_rw.assign((size_t)W * R_, 0); in.free_after.assign((size_t)W * R_, 0);
+    ids.assign(W, 0);
     uint32_t i = 0;
     bool any_blocked = false;
     for (const auto& kv : workers_) any_blocked |= !kv.second.blocked.empty();
+    blocked.clear();
     if (any_blocked) blocked.assign((size_t)W * Q, 0);
     for (const auto& kv : workers_) {                      // ascending id (solver.rs:44)
         const WorkerState& w = kv.second;
@@ -220,9 +224,29 @@ WorkerTaskMapping GpuCore::run_scheduling(uint64_t now_ms) {
             }
         hqs_prefill_state(ctx_, W, pfwc.data());
     }
+    return true;
+}
+
+// the free vectors after the tick replace the host mirror's
+void GpuCore::apply_free_after(const TickInput& in) {
+    uint32_t i = 0;
+    for (auto& kv : workers_) {
+        std::copy(in.free_after.begin() + (size_t)i * R_, in.free_after.begin() + (size_t)(i + 1) * R_, kv.second.free.begin());
+        ++i;
+    }
+}
+
+// run_scheduling_inner (main.rs:40-46): builds the per-tick worker view, runs the tick, applies the result to the
+// host mirror (Worker::insert_sn_task: free -= request; task state Waiting -> Assigned) and groups it per worker.
+WorkerTaskMapping GpuCore::run_scheduling(uint64_t now_ms) {
+    WorkerTaskMapping mapping;
+    TickInput in;
+    if (!tick_input(now_ms, in)) return mapping;
+    const uint32_t W = (uint32_t)in.hw.size();
+    const std::vector<WorkerId>& ids = in.ids;
     uint32_t n = 0;
-    const int rc = hqs_tick(ctx_, W, hw.data(), free_rw.data(), total_rw.data(), any_blocked ? blocked.data() : nullptr,
-                            (uint32_t)out_.size(), out_.data(), &n, free_after.data());
+    const int rc = hqs_tick(ctx_, W, in.hw.data(), in.free_rw.data(), in.total_rw.data(), in.blocked.empty() ? nullptr : in.blocked.data(),
+                            (uint32_t)out_.size(), out_.data(), &n, in.free_after.data());
     if (rc != HQS_OK) {                                    // the reference logs and schedules nothing (solver.rs:412-415)
         last_error_ = hqs_last_error(ctx_);
         log_error("tick failed, nothing scheduled", last_error_.c_str());
@@ -251,11 +275,7 @@ WorkerTaskMapping GpuCore::run_scheduling(uint64_t now_ms) {
         t.variant = a.variant;
         mapping.workers[ids[a.worker]].assigned.emplace_back(t.id, a.variant);     // emission order = priority desc
     }
-    i = 0;
-    for (auto& kv : workers_) {
-        std::copy(free_after.begin() + (size_t)i * R_, free_after.begin() + (size_t)(i + 1) * R_, kv.second.free.begin());
-        ++i;
-    }
+    apply_free_after(in);
     return mapping;
 }
 

@@ -12,6 +12,7 @@ parity tests and the benchmark read like the reference's own tests:
   TaskQueues::add_ready_task     taskqueue.rs:37-43         GpuScheduler.add_ready_tasks
   TaskQueue::remove              taskqueue.rs:194-216       GpuScheduler.remove_ready_tasks
   run_scheduling_inner           main.rs:40-46              GpuScheduler.run_scheduling  -> WorkerTaskMapping
+  WorkerTaskMapping::send_messages  mapping.rs:255-288      GpuScheduler.run_scheduling_grouped -> GroupedTaskMapping
   Worker::insert_sn_task         worker.rs:188-196          (free vectors come back from the device)
   task_finished / remove_sn_task reactor.rs:500-580         GpuScheduler.tasks_finished
 
@@ -97,6 +98,61 @@ class WorkerTaskMapping:
         for t, w, v, k in zip(a["task"].tolist(), a["worker"].tolist(), a["variant"].tolist(), a["kind"].tolist()):
             if k != 1:
                 out.setdefault(int(self.worker_ids[w]), []).append((t, v))
+        return out
+
+
+@dataclass
+class GroupedTaskMapping:
+    """The same tick result as WorkerTaskMapping with the records grouped by worker on the device (hqs_tick_fetch_grouped):
+    with W = len(worker_ids), worker w's prefill records are records[worker_off[2w]:worker_off[2w+1]], its assignments
+    records[worker_off[2w+1]:worker_off[2w+2]], both in emission order, and the redirect records (kind 2) are the flat tail
+    records[worker_off[2W]:worker_off[2W+1]] in emission order.  The per-worker lists are slices."""
+    records: np.ndarray                           # L.assignment_dtype; `worker` = index into worker_ids
+    worker_off: np.ndarray                        # [2W + 2] u32
+    worker_ids: np.ndarray
+    free_after: np.ndarray                        # [W][R] u64
+    retract_from: Optional[np.ndarray] = None     # for the tail's records: index of the worker the task was prefilled on
+
+    def redirects(self) -> np.ndarray:
+        nw = self.worker_ids.shape[0]
+        return self.records[int(self.worker_off[2 * nw]): int(self.worker_off[2 * nw + 1])]
+
+    def n_assigned(self) -> int:
+        return int(self.records.shape[0]) - self.n_prefilled()
+
+    def n_prefilled(self) -> int:
+        off = self.worker_off.astype(np.int64)
+        return int((off[1:-1:2] - off[0:-2:2]).sum())
+
+    def messages(self) -> Dict[int, Dict[str, list]]:
+        """What WorkerTaskMapping.messages() returns for the same tick."""
+        out: Dict[int, Dict[str, list]] = {}
+        off = self.worker_off.tolist()
+        task, variant = self.records["task"], self.records["variant"]
+        for w, wid in enumerate(self.worker_ids.tolist()):
+            p0, a0, a1 = off[2 * w], off[2 * w + 1], off[2 * w + 2]
+            if a1 > p0:
+                out[wid] = {"retracts": [], "compute": [(t, None) for t in task[p0:a0].tolist()]
+                            + list(zip(task[a0:a1].tolist(), variant[a0:a1].tolist()))}
+        if self.retract_from is not None:
+            for t, ow in zip(self.redirects()["task"].tolist(), self.retract_from.tolist()):
+                out.setdefault(int(self.worker_ids[ow]), {"retracts": [], "compute": []})["retracts"].append(t)
+        return out
+
+    def per_worker(self) -> Dict[int, List[Tuple[int, int]]]:
+        """worker_id -> [(task handle, variant)]: the worker's assignments in emission order, which is what
+        WorkerTaskMapping.per_worker() returns for a tick without redirect records.  Tasks redirected to the worker follow
+        its assignments here (the grouped layout keeps them in the tail, not at their place in the emission order)."""
+        out: Dict[int, List[Tuple[int, int]]] = {}
+        off = self.worker_off.tolist()
+        task, variant = self.records["task"], self.records["variant"]
+        for w, wid in enumerate(self.worker_ids.tolist()):
+            a0, a1 = off[2 * w + 1], off[2 * w + 2]
+            if a1 > a0:
+                out[wid] = list(zip(task[a0:a1].tolist(), variant[a0:a1].tolist()))
+        red = self.redirects()
+        for t, w, v in zip(red["task"].tolist(), red["worker"].tolist(), red["variant"].tolist()):
+            out.setdefault(int(self.worker_ids[w]), []).append((t, v))
         return out
 
 
@@ -372,6 +428,32 @@ class GpuScheduler:
         self.free = free_after
         retract_from = apply_tick_records(self, a)
         return WorkerTaskMapping(a, self.worker_ids.copy(), free_after, retract_from)
+
+    def run_scheduling_grouped(self, now: float = 0.0, out_cap: Optional[int] = None) -> GroupedTaskMapping:
+        """run_scheduling with the records grouped by worker on the device (hqs_tick_grouped): the same tick, the same
+        bookkeeping, and per-worker message lists that are slices of one array."""
+        self._sync_classes()
+        w = self._worker_structs(now)
+        nw = w.shape[0]
+        if out_cap is None:
+            out_cap = max(int(self._lib_stats().n_handles), 1)
+        if self._out.shape[0] < out_cap:
+            self._out = np.zeros(out_cap, dtype=L.assignment_dtype)
+        blocked = self._blocked_bytes()
+        free = np.ascontiguousarray(self.free)
+        total = np.ascontiguousarray(self.total)
+        free_after = np.zeros_like(free)
+        off = np.zeros(2 * nw + 2, dtype=np.uint32)
+        n = C.c_uint32(0)
+        if self._prefill[1] > 0:
+            self._check(self._lib.hqs_prefill_state(self._ctx, nw, L.ptr(self.prefill_mask())))
+        self._check(self._lib.hqs_tick_grouped(self._ctx, nw, L.ptr(w), L.ptr(free), L.ptr(total),
+                                               L.ptr(blocked) if blocked is not None else None, out_cap,
+                                               L.ptr(self._out), C.byref(n), off.size, L.ptr(off), L.ptr(free_after)))
+        a = self._out[: n.value].copy()
+        self.free = free_after
+        retract_from = apply_tick_records(self, a)      # kind-2 records keep their relative order in the grouped array
+        return GroupedTaskMapping(a, off, self.worker_ids.copy(), free_after, retract_from)
 
     def prefill_mask(self) -> np.ndarray:
         """"Worker w holds a prefilled task of class c" (Worker::prefilled_tasks) over this scheduler's tasks, the host's

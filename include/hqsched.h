@@ -197,6 +197,33 @@ int hqs_tick_launch(hqs_ctx* ctx, uint32_t n_workers, const hqs_worker* workers,
 int hqs_tick_fetch(hqs_ctx* ctx, uint32_t out_cap, hqs_assignment* out, uint32_t* out_n,
                    uint64_t* free_after);
 
+/* hqs_tick_fetch with the records regrouped by worker on the device, the shape tako sends them in (one message list per
+ * worker, WorkerTaskMapping::send_messages, mapping.rs:255-288).  With W = n_workers of the launch and n = *out_n:
+ *   out[ worker_off[2w]   .. worker_off[2w+1] )   worker w's prefill records (kind 1), in emission order
+ *   out[ worker_off[2w+1] .. worker_off[2w+2] )   worker w's assignments (kind 0), in emission order = priority descending
+ *   out[ worker_off[2W]   .. worker_off[2W+1] )   all redirect records (kind 2), in emission order, NOT grouped: the
+ *                                                 RetractTasks message goes to the worker the task was prefilled on, which
+ *                                                 only the host knows
+ *   worker_off[0] = 0, worker_off[2W+1] = n, non-decreasing, 2W + 2 entries
+ * i.e. a stable sort of what hqs_tick_fetch returns by key = kind == 2 ? 2W : 2 * worker + (kind == 0); the records keep
+ * their 8-byte form.  It fetches whatever tick is pending (hqs_tick_launch, hqs_shard_tick_launch, hqs_shard_solve_emit: a
+ * rank gets its own records grouped).  States and errors are hqs_tick_fetch's; in addition a null worker_off or
+ * off_cap < 2W + 2 returns HQS_E_INVALID and leaves the tick fetchable by either fetch.  The grouping kernels run at fetch
+ * time, so a failed tick launches nothing, and n == 0 launches nothing and returns an all-zero table.
+ *   hqs_tick_grouped     = hqs_tick_launch + hqs_tick_fetch_grouped
+ *   hqs_grouped_reserve  allocates what the grouped fetch needs for n_workers and out_cap records and loads its kernels
+ *                        (otherwise done by the first grouped fetch); contexts that wait for each other on the device call
+ *                        it before their first tick, as hqs_tick_reserve.  A context that never fetches grouped never pays.
+ *   hqs_grouped_kernel_ms  device time of the grouping kernels of the last grouped fetch, between two CUDA events on the
+ *                        context stream (hqs_set_profile on; HQS_E_STATE if there is none). */
+int hqs_tick_fetch_grouped(hqs_ctx* ctx, uint32_t out_cap, hqs_assignment* out, uint32_t* out_n, uint32_t off_cap,
+                           uint32_t* worker_off, uint64_t* free_after);
+int hqs_tick_grouped(hqs_ctx* ctx, uint32_t n_workers, const hqs_worker* workers, const uint64_t* free_rw,
+                     const uint64_t* total_rw, const uint8_t* blocked_wcv, uint32_t out_cap, hqs_assignment* out,
+                     uint32_t* out_n, uint32_t off_cap, uint32_t* worker_off, uint64_t* free_after);
+int hqs_grouped_reserve(hqs_ctx* ctx, uint32_t n_workers, uint32_t out_cap);
+int hqs_grouped_kernel_ms(hqs_ctx* ctx, float* out_ms);
+
 /* What-if query (scheduler/query.rs:12-131, ServerRef::new_worker_query control.rs:123-136): runs the histogram
  * and the solver against an arbitrary (e.g. hypothetical, autoalloc) worker array WITHOUT emitting or consuming
  * anything: the ready set is unchanged.  per_worker_assigned[n_workers] (optional) receives how many tasks each

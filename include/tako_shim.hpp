@@ -110,6 +110,10 @@ public:
     void remove_ready_task(TaskId task);
 
     WorkerTaskMapping run_scheduling(uint64_t now_ms = 0);
+    // The same tick and the same WorkerTaskMapping, list order included, with the records regrouped per worker on the
+    // device (hqs_tick_grouped): one map lookup and one reserved append per worker and section instead of a lookup and a
+    // push_back per record.  Defined in tako_shim_grouped.cpp.
+    WorkerTaskMapping run_scheduling_grouped(uint64_t now_ms = 0);
     void on_task_finished(TaskId task);
 
     // SchedulerConfig::proactive_filling_reserve / _max (scheduler/state.rs:14-21).  tako's defaults are 16 / 40; this
@@ -145,6 +149,14 @@ private:
         int64_t prefilled_on = -1;        // TaskRuntimeState::Prefilled{worker_id}
         int64_t retracting_from = -1;     // TaskRuntimeState::Retracting{worker_id}
     };
+    struct TickInput {                    // the worker view of one tick in the C ABI's form + the free vectors it returns
+        std::vector<hqs_worker> hw;
+        std::vector<uint64_t> free_rw, total_rw, free_after;
+        std::vector<uint8_t> blocked;     // empty: no blocked request
+        std::vector<WorkerId> ids;
+    };
+    bool tick_input(uint64_t now_ms, TickInput& in);
+    void apply_free_after(const TickInput& in);
     void flush_classes();
     void flush_ready();
     uint32_t handle_of(TaskId task);
@@ -172,4 +184,15 @@ extern "C" {
 // Self-test of the shim on CUDA device `device` (small scenarios restated from tests/test_scheduler_sn.rs plus a
 // zero-duration drain with a host-side replay of every placement).  Returns the number of failed checks.
 int hqshim_selftest(int device, int verbose);
+// Self-test of GpuCore::run_scheduling_grouped on CUDA device `device`: two identically loaded cores, one ticking flat and
+// one grouped, through a multi-class drain with priorities and through proactive filling with retract / redirect; every
+// tick's mappings must be equal, list order included, and so must the free vectors.  Returns the number of failed checks.
+int hqshim_selftest_grouped(int device, int verbose);
+// Measuring aid (tools/grouped_probe.py): host wall time of one tick INCLUDING the construction of the per-worker lists of a
+// WorkerTaskMapping, on a context the caller has loaded (handles stand in for TaskIds).  grouped = 0: hqs_tick and one map
+// lookup + push_back per record of the flat stream; grouped = 1: hqs_tick_grouped and one lookup + reserved append per worker,
+// as GpuCore::run_scheduling_grouped does.  Before each of the `reps` ticks the ready set is re-armed (not timed).
+// out_ms[reps] receives the times, *digest a hash of the lists of the last tick (equal for both forms).  Returns an HQS_E_* code.
+int hqshim_time_mapping(hqs_ctx* ctx, uint32_t n_workers, const hqs_worker* workers, const uint64_t* free_rw,
+                        const uint64_t* total_rw, uint32_t out_cap, int grouped, uint32_t reps, double* out_ms, uint64_t* digest);
 }
