@@ -494,9 +494,12 @@ class GpuScheduler:
         return pos
 
     def _take_resources(self, pos: int, rq_id: int, variant: int) -> None:
-        """A task of class rq_id started on worker index pos with the given variant: it takes the worker's resources."""
+        """A task of class rq_id started on worker index pos with the given variant: it takes the worker's resources.
+        An unlimited amount (HQS_AMOUNT_MAX) stays unlimited, as on the device."""
         am = self._amount_tab[rq_id, variant]
-        self.free[pos] = np.where(self._all_tab[rq_id, variant], 0, self.free[pos] - np.minimum(self.free[pos], am))
+        fr = self.free[pos]
+        taken = np.where(fr == L.HQS_AMOUNT_MAX, fr, fr - np.minimum(fr, am))
+        self.free[pos] = np.where(self._all_tab[rq_id, variant], 0, taken)
 
     def on_retract_response(self, worker_id: int, handles) -> Dict[int, List[Tuple[int, int]]]:
         """on_retract_response (server/reactor.rs:452-498): the worker gave the listed tasks back.  A task with a redirect
@@ -537,7 +540,8 @@ class GpuScheduler:
         amounts = self._amount_tab[cl, va]                       # [n][R]
         add = np.zeros_like(self.free)
         np.add.at(add, wi, amounts)
-        self.free = self.free + add
+        # an unlimited amount (HQS_AMOUNT_MAX) is never taken by a tick, so nothing comes back to it
+        self.free = np.where(self.free == L.HQS_AMOUNT_MAX, self.free, self.free + add)
         allm = self._all_tab[cl, va]                             # [n][R] bool
         if allm.any():
             ws, rs = np.nonzero(allm)

@@ -112,6 +112,8 @@ class _Tick:
         self.alls = [[tuple(d.get("all", ())) for d in vs] for vs in wl.classes]
         self.min_ms = [[int(round(d.get("min_time_s", 0.0) * 1000)) for d in vs] for vs in wl.classes]
         self.excluded = None
+        self.trace = None                        # model_tick's `trace` dict, or None
+        self.pass_no = 0
         self.touched = [False] * self.W          # the worker received something in this tick
         self.noresv = set()                      # classes for which no worker can be reserved any more
 
@@ -150,6 +152,8 @@ class _Tick:
                     continue
                 self.excluded[w] = True
                 got += 1
+                if self.trace is not None:
+                    self.trace["reserved"].append((self.pass_no, w, c))
         if got < remaining:
             self.noresv.add(c)            # eligibility only shrinks during a tick
 
@@ -175,6 +179,8 @@ class _Tick:
     def fit(self, w: int, c: int, v: int, cap: int) -> int:
         """How many tasks of (c, v) fit on worker w now, at most `cap`."""
         if not self.admissible(w, c, v):
+            if self.trace is not None and not (self.excluded is not None and self.excluded[w]):
+                self._trace_rejection(w, c, v)
             return 0
         cnt = cap
         fr, tot = self.fr[w], self.tot[w]
@@ -184,6 +190,18 @@ class _Tick:
             elif r in self.am[c][v] and fr[r] != AMOUNT_MAX:
                 cnt = min(cnt, fr[r] // self.am[c][v][r])
         return cnt
+
+    def _trace_rejection(self, w: int, c: int, v: int) -> None:
+        """Records a blocked or time-limited (worker, class, variant) cell whose resources would take a task now."""
+        fr, tot = self.fr[w], self.tot[w]
+        for r in range(self.R):
+            if r in self.alls[c][v]:
+                if not (tot[r] != 0 and fr[r] == tot[r]):
+                    return
+            elif r in self.am[c][v] and fr[r] != AMOUNT_MAX and fr[r] < self.am[c][v][r]:
+                return
+        why = "blocked" if self.wl.blocked is not None and self.wl.blocked[w, c, v] else "time"
+        self.trace["rejected"].append((why, w, c, v))
 
     def next_variant(self, w: int, c: int, tried: int) -> int:
         """The untried variant of class c that costs the smallest share of what worker w has left:
@@ -267,6 +285,11 @@ def _level_is_saturated(t: _Tick, groups: List[Tuple[int, int]], vorder: List[Li
     return n_sat > 0, phi
 
 
+def _pack_quota(n: int, cn: int, T: int, phi: float) -> int:
+    """A worker's share of a packed class: ceil(n * cn / T), scaled by phi and rounded up again."""
+    return int(math.ceil(float(-(-n * cn // T)) * phi))
+
+
 def _pack_level(t: _Tick, groups: List[Tuple[int, int]], phi: float) -> Dict[Tuple[int, int], List[int]]:
     """Every worker fills itself (its free vector is consumed).  Returns taken[(group index, variant)][w]."""
     W, R = t.W, t.R
@@ -278,7 +301,7 @@ def _pack_level(t: _Tick, groups: List[Tuple[int, int]], phi: float) -> Dict[Tup
         T = sum(cn)
         if T:
             for w in range(W):
-                quota[w][gi] = int(math.ceil(float(-(-n * cn[w] // T)) * phi))
+                quota[w][gi] = _pack_quota(n, cn[w], T, phi)
     # b. every worker fills itself
     taken: Dict[Tuple[int, int], int] = {}       # (w, candidate index) -> count
     for w in range(W):
@@ -342,19 +365,29 @@ def _pack_level(t: _Tick, groups: List[Tuple[int, int]], phi: float) -> Dict[Tup
 def model_tick(wl: Workload, ready: np.ndarray, free: np.ndarray, levels: Optional[np.ndarray] = None,
                remaining_ms: Optional[np.ndarray] = None, pack: bool = True,
                min_utilization: Optional[np.ndarray] = None, prefill: Optional[Tuple[int, int]] = None,
-               pf_worker: Optional[np.ndarray] = None) -> Tuple[np.ndarray, np.ndarray]:
+               pf_worker: Optional[np.ndarray] = None, trace: Optional[dict] = None) -> Tuple[np.ndarray, np.ndarray]:
     """Returns (assignments in device emission order, free_after).
+
+    trace: an optional dict that collects the tick's decisions (it does not change them): "reserved" [(pass, worker,
+    class)], "mu_excluded" [[workers newly excluded by pass p] ...] (one list per restart), "give_back" [(worker, class,
+    variant, count)] of pack, "variant_takes" [(worker, class, variant, try)] of first-fit takes that were not the worker's
+    first variant choice (try > 0), "rejected" [("blocked" | "time", worker, class, variant)] of cells whose resources
+    would have taken a task.
 
     min_utilization (solver.rs:154-156, 479-518): a worker either receives at least
     min_cpus = total * (mu - 1) + free cpus of new work in this tick, or nothing.  A violating worker is taken out of
     the tick and the solve starts over (at most MU_MAX_PASSES - 1 times), so its tasks go to the other workers."""
     W = free.shape[0]
     excluded = np.zeros(W, dtype=bool)
+    if trace is not None:
+        for k in ("reserved", "mu_excluded", "give_back", "variant_takes", "rejected"):
+            trace.setdefault(k, [])
     for p in range(MU_MAX_PASSES):
-        a, fa = _solve_pass(wl, ready, free, levels, remaining_ms, pack, excluded, pf_worker)
+        a, fa = _solve_pass(wl, ready, free, levels, remaining_ms, pack, excluded, pf_worker, trace, p)
         if min_utilization is None or p + 1 >= MU_MAX_PASSES:
             return _with_prefill(wl, ready, a, levels, prefill, pf_worker), fa
         viol = False
+        newly = []
         for w in range(W):
             mu = float(np.float32(min_utilization[w]))
             t0, f0 = int(wl.worker_total[w, 0]), int(free[w, 0])
@@ -365,6 +398,9 @@ def model_tick(wl: Workload, ready: np.ndarray, free: np.ndarray, levels: Option
             if min_cpus >= 0.0001 and new_cpus > 0.0 and new_cpus < min_cpus - 1e-9:
                 excluded[w] = True
                 viol = True
+                newly.append(w)
+        if trace is not None and newly:
+            trace["mu_excluded"].append(newly)
         if not viol:
             return _with_prefill(wl, ready, a, levels, prefill, pf_worker), fa
     raise AssertionError("unreachable")
@@ -419,7 +455,7 @@ def _with_prefill(wl: Workload, ready: np.ndarray, a: np.ndarray, levels, prefil
         if size <= 0:
             continue
         got = np.unique(out["worker"][(out["kind"] == 0) & (wl.task_class[out["task"]] == c)])
-        elig = [int(w) for w in got.tolist() if not np.any((pf_start == w) & ready & (wl.task_class == c))]
+        elig = [int(w) for w in got.tolist() if not _holds_prefill(pf_start, ready, wl.task_class, w, c)]
         if not elig:
             continue
         ps = min(size // len(elig), pmax)
@@ -436,11 +472,17 @@ def _with_prefill(wl: Workload, ready: np.ndarray, a: np.ndarray, levels, prefil
     return out
 
 
+def _holds_prefill(pf_start: np.ndarray, ready: np.ndarray, task_class: np.ndarray, w: int, c: int) -> bool:
+    """Worker w held a prefilled task of class c at tick start (Worker::prefilled_tasks, the host's mirror)."""
+    return bool(np.any((pf_start == w) & ready & (task_class == c)))
+
+
 MU_MAX_PASSES = 8
 
 
 def _solve_pass(wl: Workload, ready: np.ndarray, free: np.ndarray, levels, remaining_ms, pack: bool,
-                excluded: np.ndarray, pf_worker: Optional[np.ndarray] = None) -> Tuple[np.ndarray, np.ndarray]:
+                excluded: np.ndarray, pf_worker: Optional[np.ndarray] = None, trace: Optional[dict] = None,
+                pass_no: int = 0) -> Tuple[np.ndarray, np.ndarray]:
     W, R = free.shape
     prio = wl.task_user_priority.astype(np.int64)
     if levels is None:
@@ -449,6 +491,7 @@ def _solve_pass(wl: Workload, ready: np.ndarray, free: np.ndarray, levels, remai
         remaining_ms = wl.remaining_ms()
     t = _Tick(wl, free, remaining_ms)
     t.excluded = [bool(x) for x in excluded]
+    t.trace, t.pass_no = trace, pass_no
     # reservations can only exist when some worker is partly occupied at tick start (free != total)
     t.any_partial = any(t.fr0[w][r] != t.tot[w][r] for w in range(W) for r in range(R))
     order = class_order(wl, free, wl.worker_total)
@@ -484,8 +527,20 @@ def _solve_pass(wl: Workload, ready: np.ndarray, free: np.ndarray, levels, remai
             if n_cand <= PACK_MAX_CAND and len(groups) <= PACK_MAX_CAND and not has_all:
                 saturated, phi = _level_is_saturated(t, groups, vorder)
                 if saturated:
+                    before = list(t.touched)
                     taken = _pack_level(t, groups, phi)
                     packed = True
+                    # a worker whose pack takes are all handed back below received no assignment: it can still be
+                    # reserved.  The capping of every group is known now, so `touched` is what the workers keep.
+                    t.touched = before
+                    for gi, (c, n) in enumerate(groups):
+                        pos = 0
+                        for v in range(len(t.am[c])):
+                            for w, k in enumerate(taken[(gi, v)]):
+                                use = min(k, n - pos)
+                                if use > 0:
+                                    t.touched[w] = True
+                                    pos += use
         for gi, (c, n) in enumerate(groups):
             tasks = tasks_of[gkeys[gi]]
             pos = 0
@@ -502,6 +557,8 @@ def _solve_pass(wl: Workload, ready: np.ndarray, free: np.ndarray, levels, remai
                     use = min(k, n - pos)
                     if use < k:
                         t.give_back(w, c, v, k - use)
+                        if trace is not None:
+                            trace["give_back"].append((w, c, v, k - use))
                     for tt in tasks[pos: pos + use].tolist():
                         out.append((tt, w, v, 0))
                     pos += use
@@ -520,6 +577,8 @@ def _solve_pass(wl: Workload, ready: np.ndarray, free: np.ndarray, levels, remai
                     if cnt <= 0:
                         continue
                     t.take(w, c, v, cnt)
+                    if trace is not None and vi:
+                        trace["variant_takes"].append((w, c, v, vi))
                     for tt in tasks[pos: pos + cnt].tolist():
                         out.append((tt, w, v, 0))
                     pos += cnt
