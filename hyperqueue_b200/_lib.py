@@ -28,6 +28,7 @@ ABI_SYMBOLS = [
     "hqs_prefill_config", "hqs_prefill_state", "hqs_prefill_dispose", "hqs_ready_push_range", "hqs_debug_keys",
     "hqs_query_fetch", "hqs_shard_query_launch", "hqs_shard_query_solve",
     "hqs_tick_fetch_grouped", "hqs_tick_grouped", "hqs_grouped_reserve", "hqs_grouped_kernel_ms",
+    "hqs_levels_live", "hqs_levels_retain",
 ]
 HQS_IPC_HANDLE_BYTES = 64
 
@@ -147,6 +148,8 @@ def load_library() -> C.CDLL:
     lib.hqs_debug_read.argtypes = [vp, C.POINTER(C.c_uint64)]
     lib.hqs_debug_keys.argtypes = [vp, u32, u32p, C.POINTER(C.c_uint32)]
     lib.hqs_levels_add.argtypes = [vp, u32, u64p]
+    lib.hqs_levels_live.argtypes = [vp, u32, u64p, u8p, C.POINTER(C.c_uint32)]
+    lib.hqs_levels_retain.argtypes = [vp, u32, u8p]
     lib.hqs_query.argtypes = [vp, u32, vp, u64p, u64p, u8p, C.POINTER(C.c_uint32), u32p, u64p]
     lib.hqs_query_fetch.argtypes = [vp, C.POINTER(C.c_uint32), u32p, u64p]
     lib.hqs_shard_query_launch.argtypes = [vp, u32, vp, u64p, u64p, u8p]

@@ -254,14 +254,11 @@ int relevel_all(hqs_ctx* ctx) {
     return HQS_OK;
 }
 
-// Drops the priority levels no task of the table carries any more (tako priorities have a per-job component, so a
-// long-running server sees one level per job ever submitted).  Called when the level set is about to exceed what the
-// group limit allows, or has doubled since the last pruning.  Returns true if levels were dropped (the caller then
-// uploads the table and re-keys the tasks).
-int prune_levels(hqs_ctx* ctx, bool* changed) {
-    *changed = false;
+// For every exact level of ctx->levels, whether a VALID key carries its priority (one level_live_k pass over the table).
+int live_levels(hqs_ctx* ctx, std::vector<u32>& live) {
     const u32 L = (u32)ctx->levels.size();
-    if (ctx->levels_declared || L == 0 || ctx->n_handles == 0) return HQS_OK;
+    live.assign(L, 0);
+    if (L == 0 || ctx->n_handles == 0) return HQS_OK;
     // scratch kept across calls: a coarse table is pruned on every push that brings a new priority, and cudaFree would
     // synchronise the device each time
     if (L > ctx->prune_cap) {
@@ -278,9 +275,23 @@ int prune_levels(hqs_ctx* ctx, bool* changed) {
     CU(cudaMemcpyAsync(d_lv, ctx->levels.data(), (size_t)L * 8, cudaMemcpyHostToDevice, ctx->stream));
     level_live_k<<<(ctx->n_handles + 255) / 256, 256, 0, ctx->stream>>>(ctx->n_handles, ctx->d_key, ctx->d_prio, d_lv, L, d_live);
     ctx->stats.kernel_launches++;
-    std::vector<u32> live(L);
     CU(cudaMemcpyAsync(live.data(), d_live, (size_t)L * 4, cudaMemcpyDeviceToHost, ctx->stream));
     CU(cudaStreamSynchronize(ctx->stream));
+    return HQS_OK;
+}
+
+// Drops the priority levels no task of the table carries any more (tako priorities have a per-job component, so a
+// long-running server sees one level per job ever submitted).  Called when the level set is about to exceed what the
+// group limit allows, or has doubled since the last pruning.  Returns true if levels were dropped (the caller then
+// uploads the table and re-keys the tasks).  Declared levels are pruned by the caller, over all ranks
+// (hqs_levels_live / hqs_levels_retain).
+int prune_levels(hqs_ctx* ctx, bool* changed) {
+    *changed = false;
+    const u32 L = (u32)ctx->levels.size();
+    if (ctx->levels_declared || L == 0 || ctx->n_handles == 0) return HQS_OK;
+    std::vector<u32> live;
+    int rc = live_levels(ctx, live);
+    if (rc) return rc;
     std::vector<u64> kept;
     kept.reserve(L);
     for (u32 i = 0; i < L; ++i)
@@ -1175,6 +1186,49 @@ int hqs_levels_add(hqs_ctx* ctx, uint32_t n, const uint64_t* priority) {
     if (!merge_levels(ctx, fresh)) return HQS_OK;
     int rc = upload_levels(ctx);
     if (rc) return rc;
+    return relevel_all(ctx);
+}
+
+int hqs_levels_live(hqs_ctx* ctx, uint32_t cap, uint64_t* levels, uint8_t* live, uint32_t* n_levels) {
+    if (!ctx) return HQS_E_INVALID;
+    if (ctx->tick_pending) return fail(ctx, HQS_E_STATE, "the previous tick has not been fetched");
+    if (cap && (!levels || !live)) return fail(ctx, HQS_E_INVALID, "null level arrays");
+    const u32 L = (u32)ctx->levels.size();
+    if (n_levels) *n_levels = L;
+    if (!cap) return HQS_OK;
+    if (cap < L) return fail(ctx, HQS_E_INVALID, "cap=%u < n_levels=%u", cap, L);
+    CU(cudaSetDevice(ctx->device));
+    std::vector<u32> lv;
+    int rc = live_levels(ctx, lv);
+    if (rc) return rc;
+    for (u32 i = 0; i < L; ++i) {
+        levels[i] = ctx->levels[i];
+        live[i] = lv[i] ? 1 : 0;
+    }
+    return HQS_OK;
+}
+
+int hqs_levels_retain(hqs_ctx* ctx, uint32_t n, const uint8_t* keep) {
+    if (!ctx) return HQS_E_INVALID;
+    if (ctx->tick_pending) return fail(ctx, HQS_E_STATE, "the previous tick has not been fetched");
+    const u32 L = (u32)ctx->levels.size();
+    if (n != L) return fail(ctx, HQS_E_INVALID, "n=%u != n_levels=%u", n, L);
+    if (L && !keep) return fail(ctx, HQS_E_INVALID, "null keep array");
+    CU(cudaSetDevice(ctx->device));
+    std::vector<u32> lv;
+    int rc = live_levels(ctx, lv);
+    if (rc) return rc;
+    std::vector<u64> kept;
+    kept.reserve(L);
+    for (u32 i = 0; i < L; ++i) {
+        if (keep[i]) kept.push_back(ctx->levels[i]);
+        else if (lv[i]) return fail(ctx, HQS_E_INVALID, "level %u (priority %llu) is carried by a task of this context", i,
+                                    (unsigned long long)ctx->levels[i]);
+    }
+    ctx->levels_pruned_at = kept.size();
+    if (kept.size() == L) return HQS_OK;
+    ctx->levels.swap(kept);
+    if ((rc = upload_levels(ctx))) return rc;
     return relevel_all(ctx);
 }
 

@@ -182,6 +182,24 @@ def apply_tick_records(s, a: np.ndarray) -> Optional[np.ndarray]:
     return retract_from
 
 
+def return_resources(s, h: np.ndarray) -> None:
+    """The host's bookkeeping of task_finished (Worker::remove_sn_task -> WorkerResources::add, workerload.rs:194-202) on
+    the scheduler `s` whose task handles `h` are (a GpuScheduler, or the owner rank's one of a sharded ready set): each
+    task's amounts go back to the worker it ran on, an `All` resource gets the worker's total back, and the tasks are no
+    longer assigned.  An unlimited amount (HQS_AMOUNT_MAX) is never taken by a tick, so nothing comes back to it."""
+    wi = s._task_worker[h]
+    cl = s._task_class[h]
+    va = s._task_variant[h]
+    add = np.zeros_like(s.free)
+    np.add.at(add, wi, s._amount_tab[cl, va])                 # [n][R] summed per worker
+    s.free = np.where(s.free == L.HQS_AMOUNT_MAX, s.free, s.free + add)
+    allm = s._all_tab[cl, va]                                 # [n][R] bool
+    if allm.any():
+        ws, rs = np.nonzero(allm)
+        s.free[wi[ws], rs] = s.total[wi[ws], rs]
+    s._task_worker[h] = -1
+
+
 def query_workers(worker_totals: np.ndarray, remaining_s: Optional[np.ndarray] = None,
                   min_utilization: Optional[np.ndarray] = None) -> Tuple[np.ndarray, np.ndarray]:
     """The fake-worker array of a what-if query (new_worker_query): worker ids 0..n-1, time limits in seconds (inf = none)
@@ -534,19 +552,7 @@ class GpuScheduler:
         h = np.ascontiguousarray(handles, dtype=np.uint32)
         if h.size == 0:
             return 0
-        wi = self._task_worker[h]
-        cl = self._task_class[h]
-        va = self._task_variant[h]
-        amounts = self._amount_tab[cl, va]                       # [n][R]
-        add = np.zeros_like(self.free)
-        np.add.at(add, wi, amounts)
-        # an unlimited amount (HQS_AMOUNT_MAX) is never taken by a tick, so nothing comes back to it
-        self.free = np.where(self.free == L.HQS_AMOUNT_MAX, self.free, self.free + add)
-        allm = self._all_tab[cl, va]                             # [n][R] bool
-        if allm.any():
-            ws, rs = np.nonzero(allm)
-            self.free[wi[ws], rs] = self.total[wi[ws], rs]
-        self._task_worker[h] = -1
+        return_resources(self, h)
         if propagate:
             n_new = C.c_uint32(0)
             self._check(self._lib.hqs_tasks_finished(self._ctx, h.size, L.ptr(h), C.byref(n_new)))
@@ -566,6 +572,29 @@ class GpuScheduler:
         n = C.c_uint32(0)
         self._check(self._lib.hqs_query(self._ctx, nw, L.ptr(w), L.ptr(tot), L.ptr(tot), None, C.byref(n), L.ptr(counts), None))
         return counts > 0, counts, int(n.value)
+
+    # declared priority levels (sharded ready sets) ------------------------------------------------
+    def n_declared_levels(self) -> int:
+        n = C.c_uint32(0)
+        self._check(self._lib.hqs_levels_live(self._ctx, 0, None, None, C.byref(n)))
+        return int(n.value)
+
+    def levels_live(self) -> Tuple[np.ndarray, np.ndarray]:
+        """The context's exact level table (u64, descending) and, per level, whether a task of this context carries it
+        (uint8 0 / 1)."""
+        n = self.n_declared_levels()
+        lv = np.zeros(n, dtype=np.uint64)
+        live = np.zeros(n, dtype=np.uint8)
+        if n:
+            got = C.c_uint32(0)
+            self._check(self._lib.hqs_levels_live(self._ctx, n, L.ptr(lv), L.ptr(live), C.byref(got)))
+        return lv, live
+
+    def levels_retain(self, keep: np.ndarray) -> None:
+        """Drops the levels whose entry of `keep` (aligned with levels_live()) is 0; none of them may be carried by a task
+        of this context."""
+        k = np.ascontiguousarray(keep, dtype=np.uint8)
+        self._check(self._lib.hqs_levels_retain(self._ctx, k.size, L.ptr(k)))
 
     # misc ---------------------------------------------------------------------------------------
     def rearm(self) -> None:

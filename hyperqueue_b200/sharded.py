@@ -20,12 +20,16 @@ solver kernel acquires all flags and sums the vectors itself (hqs_shard_tick_lau
 used once, at set-up, to pass the 64-byte IPC handles around.
 
 Proactive filling works in both forms.  Each rank keeps the prefill state of its own tasks; before the tick the ranks OR
-their "worker holds a prefilled task of the class" masks (reduce_prefill_mask), so every rank solves with the same global
+their "worker holds a prefilled task of the class" masks (reduce_or), so every rank solves with the same global
 mask, computes the same prefill ranges and emits the prefill records of its own tasks.
 
 The autoalloc what-if query (ShardedScheduler.new_worker_query) runs the same two forms without the emit step
 (hqs_shard_query_launch, or hqs_shard_count + exchange + hqs_shard_query_solve): every rank solves the summed counts and
 returns the same answer, the one a single context holding all ranks' tasks gives.
+
+Priority levels are declared on every rank (hqs_levels_add), so that every rank numbers them identically, and are pruned
+by all ranks together at the start of a tick or a query (ShardedScheduler.prune_levels): a level is dropped only when no
+task of any rank carries it.
 """
 from __future__ import annotations
 
@@ -37,7 +41,7 @@ import torch
 import torch.distributed as dist
 
 from . import _lib as L
-from .scheduler import WorkerTaskMapping, apply_tick_records, query_workers
+from .scheduler import WorkerTaskMapping, apply_tick_records, query_workers, return_resources
 
 
 def shard_exchange(counts_local: torch.Tensor, rank: int, world: int,
@@ -53,18 +57,31 @@ def shard_exchange(counts_local: torch.Tensor, rank: int, world: int,
     return counts_all, before
 
 
-def reduce_prefill_mask(mask_local: np.ndarray, world: int, group: Optional[dist.ProcessGroup] = None,
-                        device: Optional[torch.device] = None) -> np.ndarray:
-    """Proactive filling in a sharded tick: "worker w holds a prefilled task of class c" must hold over the tasks of ALL
-    ranks, but each rank knows only its own prefilled tasks.  Returns the OR of the ranks' uint8 [W][Q] masks (one
-    all-reduce, on `device` for NCCL); every rank passes the result to hqs_prefill_state."""
-    m = np.ascontiguousarray(mask_local, dtype=np.uint8)
+def reduce_or(local: np.ndarray, world: int, group: Optional[dist.ProcessGroup] = None,
+              device: Optional[torch.device] = None) -> np.ndarray:
+    """The element-wise OR of the ranks' uint8 0 / 1 arrays of one shape (one all-reduce, on `device` for NCCL).  Used for
+    what must hold over the tasks of ALL ranks while each rank knows only its own: "worker w holds a prefilled task of
+    class c" (the [W][Q] mask every rank passes to hqs_prefill_state) and "a task carries priority level i" (the live
+    vector every rank passes to hqs_levels_retain)."""
+    m = np.ascontiguousarray(local, dtype=np.uint8)
     if world == 1:
         return m
     dev = device if device is not None and dist.get_backend(group) == "nccl" else torch.device("cpu")
     t = torch.from_numpy(m.copy()).to(dev)
     dist.all_reduce(t, op=dist.ReduceOp.MAX, group=group)
     return np.ascontiguousarray(t.cpu().numpy())
+
+
+reduce_prefill_mask = reduce_or          # the name the prefill path has always imported
+
+
+def levels_need_pruning(n_levels: int, n_classes: int, prefill: bool, pruned_at: int) -> bool:
+    """A sharded ready set declares every priority it is given (hqs_levels_add) and never prunes on its own.  The ranks
+    prune together when the declared table exceeds what a tick's groups allow (HQS_MAX_GROUPS / Q levels, half of that
+    with proactive filling, which doubles the groups) or has more than doubled (+64) since the last pruning.  Declared
+    tables are identical on every rank, so every rank decides the same way."""
+    budget = L.HQS_MAX_GROUPS // (max(n_classes, 1) * (2 if prefill else 1))
+    return n_levels > budget or n_levels > 2 * pruned_at + 64
 
 
 def gather_peer_handles(sched, rank: int, world: int, group: Optional[dist.ProcessGroup] = None):
@@ -126,6 +143,7 @@ class ShardedScheduler:
         self._counts = torch.zeros(L.HQS_MAX_GROUPS, dtype=torch.int32, device=device)
         self.p2p = bool(p2p)
         self.last_mapping: Optional[WorkerTaskMapping] = None
+        self.levels_pruned_at = 0           # declared table size after the last pruning (the same on every rank)
         if self.p2p:
             attach_peers(sched, rank, world, group)
 
@@ -139,12 +157,33 @@ class ShardedScheduler:
         if m.any():
             self.s.add_ready_tasks((h[m] - self.lo).astype(np.uint32), np.asarray(rq_ids)[m], np.asarray(priorities)[m])
 
+    def remove_ready_tasks(self, handles) -> None:
+        """TaskQueue::remove for GLOBAL handles, called with the same list on every rank: the owner of each task takes it
+        out of its ready set.  Also the way to retire the handle of a finished task, so that it no longer keeps its
+        priority level alive (prune_levels)."""
+        mine = self._mine(handles)
+        if mine.size:
+            self.s.remove_ready_tasks(mine.astype(np.uint32))
+
+    def prune_levels(self) -> None:
+        """Drops the declared priority levels that no task of any rank carries (levels_need_pruning decides when; a
+        collective when it does).  Called at the start of run_scheduling and new_worker_query, where no tick is in flight."""
+        s = self.s
+        n = s.n_declared_levels()
+        if not levels_need_pruning(n, s.n_classes, s._prefill[1] > 0, self.levels_pruned_at):
+            return
+        _, live = s.levels_live()
+        keep = reduce_or(live, self.world, self.group, self.device)
+        s.levels_retain(keep)
+        self.levels_pruned_at = int(np.count_nonzero(keep))
+
     def run_scheduling(self, now: float = 0.0, out_cap: Optional[int] = None):
         """One sharded tick.  Returns (this rank's records with GLOBAL handles, free vectors after the tick): its assignments
         (kind 0 / 2) in single-context order, then its prefill records (kind 1).  self.last_mapping holds the same records
         as a WorkerTaskMapping (messages(), retracts of kind-2 records)."""
         s = self.s
         s._sync_classes()
+        self.prune_levels()
         w = s._worker_structs(now)
         free = np.ascontiguousarray(s.free)
         total = np.ascontiguousarray(s.total)
@@ -152,7 +191,7 @@ class ShardedScheduler:
         if s._prefill[1] > 0:
             # a host collective at tick start: the previous tick has been fetched, so no collective overlaps a tick in
             # flight (DESIGN.md §6); every rank passes the same global mask
-            pfwc = reduce_prefill_mask(s.prefill_mask(), self.world, self.group, self.device)
+            pfwc = reduce_or(s.prefill_mask(), self.world, self.group, self.device)
             s._check(s._lib.hqs_prefill_state(s._ctx, w.shape[0], L.ptr(pfwc)))
         cap = out_cap or max(self.hi - self.lo, 1)
         if self.p2p:
@@ -185,6 +224,7 @@ class ShardedScheduler:
         (DESIGN.md §6).  `now` is accepted for symmetry with GpuScheduler: the fake workers' time limits are remaining_s."""
         s = self.s
         s._sync_classes()
+        self.prune_levels()
         w, tot = query_workers(worker_totals, remaining_s, min_utilization)
         nw = tot.shape[0]
         if self.p2p:
@@ -255,28 +295,19 @@ class ShardedScheduler:
 
     def tasks_finished(self, handles) -> None:
         """task_finished for GLOBAL handles, called with the same list on every rank: every rank holds the replicated free
-        vectors, but only the owner of a task knows where it ran, so the per-worker amounts to give back are summed over the
-        ranks (one all-reduce of a [W][R] matrix, or nothing with world == 1)."""
+        vectors, but only the owner of a task knows where it ran.  The owner returns the resources as GpuScheduler does
+        (scheduler.return_resources: an unlimited amount stays unlimited, `All` gives the total back), and the per-worker change of its
+        free vectors is summed over the ranks (one all-reduce of a [W][R] matrix, or nothing with world == 1)."""
         s = self.s
-        h = np.asarray(handles, dtype=np.int64)
-        mine = h[(h >= self.lo) & (h < self.hi)] - self.lo
-        add = np.zeros_like(s.free)
-        reset = np.zeros(s.free.shape, dtype=bool)
+        mine = self._mine(handles)
+        before = s.free.copy()
         if mine.size:
-            wi, cl, va = s._task_worker[mine], s._task_class[mine], s._task_variant[mine]
-            assert (wi >= 0).all(), "a finished task of this rank was never assigned"
-            np.add.at(add, wi, s._amount_tab[cl, va])
-            allm = s._all_tab[cl, va]
-            if allm.any():
-                ws, rs = np.nonzero(allm)
-                reset[wi[ws], rs] = True
-            s._task_worker[mine] = -1
+            assert (s._task_worker[mine] >= 0).all(), "a finished task of this rank was never assigned"
+            return_resources(s, mine)
         if self.world > 1:
-            t = torch.from_numpy(np.stack([add.astype(np.int64), reset.astype(np.int64)]))
+            # finishing only adds to a free vector: the change is >= 0 and below the worker's total
+            delta = (s.free - before).view(np.int64)
             dev = self.device if dist.get_backend(self.group) == "nccl" else torch.device("cpu")
-            t = t.to(dev)
+            t = torch.from_numpy(np.ascontiguousarray(delta)).to(dev)
             dist.all_reduce(t, group=self.group)
-            t = t.cpu().numpy()
-            add, reset = t[0].astype(np.uint64), t[1] > 0
-        s.free = s.free + add.astype(np.uint64)
-        s.free[reset] = s.total[reset]
+            s.free = before + t.cpu().numpy().view(np.uint64)

@@ -155,8 +155,18 @@ int hqs_ready_push(hqs_ctx* ctx, uint32_t n, const uint32_t* task, const uint32_
 int hqs_ready_push_range(hqs_ctx* ctx, uint32_t first_task, uint32_t n, const uint32_t* class_id, const uint64_t* priority);
 /* Declares priority values before any task carries them.  Needed when the ready set is sharded over
  * several contexts (every rank must number the priority levels identically).  A context whose levels were declared
- * does not prune them on its own (the ranks would diverge). */
+ * does not prune them on its own (the ranks would diverge): the caller prunes them over all ranks with
+ * hqs_levels_live and hqs_levels_retain, between ticks. */
 int hqs_levels_add(hqs_ctx* ctx, uint32_t n, const uint64_t* priority);
+/* The context's exact level table (registered priorities, descending) and, per level, whether a VALID key of this
+ * context carries it (1) or not (0).  *n_levels (optional) receives the table size; with cap == 0 nothing else is done,
+ * otherwise cap must be >= the table size.  A level dead on this rank may be live on another: the ranks OR their live
+ * vectors before hqs_levels_retain.  HQS_E_STATE while a tick has not been fetched. */
+int hqs_levels_live(hqs_ctx* ctx, uint32_t cap, uint64_t* levels, uint8_t* live, uint32_t* n_levels);
+/* Keeps the levels with keep[i] != 0 (i indexes the table hqs_levels_live returned), drops the others, rebuilds the
+ * device table and re-keys every VALID task.  HQS_E_INVALID, with nothing changed, if n is not the table size or a
+ * dropped level is still carried by a VALID key of this context.  Every rank must pass the same keep vector. */
+int hqs_levels_retain(hqs_ctx* ctx, uint32_t n, const uint8_t* keep);
 /* TaskQueue::remove (taskqueue.rs:194-216): cancel / externally assigned tasks leave the ready set.  Also the way to
  * retire the handle of a task that has FINISHED: a removed handle leaves the device table, so it no longer pins its
  * priority level (levels without any task are pruned when the level set outgrows HQS_MAX_GROUPS / n_classes or doubles;

@@ -392,6 +392,28 @@ class Drain:
         return out
 
 
+def gpu_context(d: Drain, flags: int = 0):
+    """A GpuScheduler set up as the scenario's server: classes, workers, termination, min-utilisation, blocked mask,
+    proactive filling; `flags` are hqs_create flags (NO_PACK follows the scenario)."""
+    from hyperqueue_b200 import GpuScheduler, RequestVariant, _lib as L
+    sc = d.sc
+    s = GpuScheduler(sc.R, 0, flags | (0 if sc.pack else L.HQS_CREATE_NO_PACK))
+    for c, vs in enumerate(sc.classes):
+        rid = s.get_or_create_resource_rq_id([RequestVariant.of(v["amounts"], v.get("all", ()), v.get("weight", 1.0),
+                                                                v.get("min_time_s", 0.0)) for v in vs])
+        assert rid == c
+    s.new_workers_bulk(np.arange(sc.W, dtype=np.uint32), sc.total)
+    s.termination = sc.termination.copy()
+    if sc.min_util is not None:
+        s.min_utilization = sc.min_util.copy()
+    if d.blocked is not None:
+        s.set_blocked_mask(d.blocked)
+    if sc.prefill is not None:
+        s.set_prefill(*sc.prefill)
+    s._sync_classes()
+    return s
+
+
 # --- checks shared by the CPU and GPU tests --------------------------------------------------------------------------
 def judge_and_replay(d: Drain, inp: TickInputs, a: np.ndarray, free_after: np.ndarray) -> Optional[str]:
     """The tick's assignments (kind 0 and 2) are feasible, no handle is placed twice, prefill records name ready tasks

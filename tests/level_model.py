@@ -17,6 +17,10 @@ The policy:
     of the bucket) and the last entry 0 (coarse: a key's level is the first bucket whose bound is <= its priority).
   * hqs_classes_set with another Q prunes (same triggers), rebuilds and re-levels; hqs_levels_add registers without ever
     pruning; hqs_dag_load replaces the table and registers exactly the DAG's priorities.
+  * hqs_levels_live returns the registered list and, per entry, whether a VALID key carries it; hqs_levels_retain(keep)
+    (the caller's pruning of declared levels, over all ranks) rejects a keep vector of another length or one that drops
+    a carried level; otherwise it drops the unflagged levels, sets the size after the last pruning, and when something
+    was dropped rebuilds the device table and re-levels every VALID key.
 Levels are only ever written into VALID keys; a key that leaves the table keeps its level and class bits.
 """
 from __future__ import annotations
@@ -203,6 +207,24 @@ class LevelModel:
             self._upload()
             self._relevel()
 
+    def levels_live(self):
+        """(registered priorities, descending; uint8 flag per entry: a VALID key carries it)."""
+        live = set(int(p) for p in self.live_priorities().tolist()) if self.n_handles else set()
+        return (np.array(self.levels, dtype=np.uint64),
+                np.array([1 if p in live else 0 for p in self.levels], dtype=np.uint8))
+
+    def levels_retain(self, keep) -> None:
+        k = np.asarray(keep, dtype=np.uint8)
+        _, live = self.levels_live()
+        if k.size != len(self.levels) or (live.astype(bool) & (k == 0)).any():
+            raise Rejected()
+        kept = [p for p, f in zip(self.levels, k.tolist()) if f]
+        self.pruned_at = len(kept)
+        if len(kept) != len(self.levels):
+            self.levels = kept
+            self._upload()
+            self._relevel()
+
     def dag_load(self, cls, prio, n_deps, cons_off, cons) -> None:
         c = np.asarray(cls, dtype=np.uint32)
         if self.Q == 0 or int(c.max()) >= self.Q:
@@ -280,7 +302,9 @@ def _pool(used: set) -> np.ndarray:
 
 def random_op(rng, m: LevelModel, used: set, declared: bool, max_q: int = 4096, few_priorities: bool = False):
     """One call for a non-DAG context in state m: ("push", handles, classes, priorities, as_range), ("remove", handles),
-    ("tick",), ("remove_done",), ("rearm",), ("dispose", class), ("classes", Q) or ("levels_add", priorities).  `used`
+    ("tick",), ("remove_done",), ("rearm",), ("dispose", class), ("classes", Q), ("levels_add", priorities) or, once
+    levels were declared, ("levels_retain", keep) with keep = the live flags of levels_live() OR some dead levels another
+    rank would still hold, and now and then a keep vector that drops a live level or has the wrong length (rejected).  `used`
     collects every priority handed out so far.  few_priorities: a batch brings at most one new priority, so that levels
     hold many tasks (proactive filling needs more waiting tasks in a level than its reserve)."""
     r = rng.random()
@@ -334,9 +358,18 @@ def random_op(rng, m: LevelModel, used: set, declared: bool, max_q: int = 4096, 
         return ("rearm",)
     if r < 0.87:
         return ("dispose", int(rng.integers(0, m.Q)))
-    if r < 0.94 or not declared:
+    if r < 0.91 or not declared:
         q = min(max_q, m.Q + int(rng.choice([1, 1, 3, 7])))
         return ("classes", q)
+    if r < 0.95 and m.declared:
+        _, live = m.levels_live()
+        keep = live | (rng.random(live.size) < rng.choice([0.0, 0.1, 0.5])).astype(np.uint8)
+        u = rng.random()
+        if u < 0.08 and live.any():
+            keep[int(rng.choice(np.nonzero(live)[0]))] = 0          # drops a level a task carries
+        elif u < 0.12:
+            keep = np.concatenate([keep, [1]]).astype(np.uint8)   # not the table's length
+        return ("levels_retain", keep)
     k = int(rng.choice([1, 10, 500]))
     return ("levels_add", np.array(_fresh_priorities(rng, k, used) + [int(x) for x in rng.choice(_pool(used), k)],
                                    dtype=np.uint64))

@@ -14,25 +14,8 @@ SEEN: dict = {}          # seed -> per-seed summary (loop bits per context, reco
 
 
 def _contexts(d: D.Drain):
-    from hyperqueue_b200 import GpuScheduler, RequestVariant, _lib as L
-    sc = d.sc
-    out = []
-    for wide in (0, L.HQS_CREATE_WIDE_AMOUNTS):
-        s = GpuScheduler(sc.R, 0, wide | (0 if sc.pack else L.HQS_CREATE_NO_PACK))
-        for c, vs in enumerate(sc.classes):
-            rid = s.get_or_create_resource_rq_id([RequestVariant.of(v["amounts"], v.get("all", ()), v.get("weight", 1.0),
-                                                                    v.get("min_time_s", 0.0)) for v in vs])
-            assert rid == c
-        s.new_workers_bulk(np.arange(sc.W, dtype=np.uint32), sc.total)
-        s.termination = sc.termination.copy()
-        if sc.min_util is not None:
-            s.min_utilization = sc.min_util.copy()
-        if d.blocked is not None:
-            s.set_blocked_mask(d.blocked)
-        if sc.prefill is not None:
-            s.set_prefill(*sc.prefill)
-        out.append(s)
-    return out
+    from hyperqueue_b200 import _lib as L
+    return [D.gpu_context(d, wide) for wide in (0, L.HQS_CREATE_WIDE_AMOUNTS)]
 
 
 def run_seed(seed: int) -> dict:

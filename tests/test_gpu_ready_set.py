@@ -202,6 +202,23 @@ class Harness:
         self._both(lambda: self.m.levels_add(p), lambda d: d.ok(d.lib.hqs_levels_add(d.ctx, p.size, d.L.ptr(p))),
                    f"levels_add of {p.size}")
 
+    def levels_retain(self, keep):
+        """hqs_levels_live on every context must equal the model's before the retain."""
+        want_lv, want_live = self.m.levels_live()
+        for d in self.devs:
+            n = C.c_uint32(0)
+            d.ok(d.lib.hqs_levels_live(d.ctx, 0, None, None, C.byref(n)))
+            assert n.value == want_lv.size, ("n_levels", n.value, want_lv.size)
+            lv, live = np.zeros(n.value, np.uint64), np.zeros(n.value, np.uint8)
+            if n.value:
+                d.ok(d.lib.hqs_levels_live(d.ctx, n.value, d.L.ptr(lv), d.L.ptr(live), C.byref(n)))
+            assert np.array_equal(lv, want_lv) and np.array_equal(live, want_live), "levels_live"
+        keep = np.ascontiguousarray(keep, np.uint8)
+        self.seen["retained"] = self.seen.get("retained", 0) + 1
+        self._both(lambda: self.m.levels_retain(keep),
+                   lambda d: d.ok(d.lib.hqs_levels_retain(d.ctx, keep.size, d.L.ptr(keep))),
+                   f"levels_retain of {keep.size} ({int(keep.size - keep.sum())} dropped)")
+
     def dag_load(self, cls, prio, n_deps, off, cons):
         arrs = [np.ascontiguousarray(cls, np.uint32), np.ascontiguousarray(prio, np.uint64),
                 np.ascontiguousarray(n_deps, np.uint32), np.ascontiguousarray(off, np.uint32),
@@ -386,6 +403,8 @@ def _run_random(h, rng, declared, n_ops, max_q=4096, few_priorities=False):
             h.classes(op[1])
         elif op[0] == "levels_add":
             h.levels_add(op[1])
+        elif op[0] == "levels_retain":
+            h.levels_retain(op[1])
 
 
 @pytest.mark.parametrize("seed", range(30))

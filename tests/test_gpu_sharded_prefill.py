@@ -35,18 +35,24 @@ def _sched(R, classes, flags=0, prefill=None):
 
 
 class Ranks:
-    """The ranks of a sharded ready set as contexts of this process; rank r owns [cuts[r], cuts[r + 1]).  The host half
-    follows ShardedScheduler: the prefill mask is the OR of the ranks' masks, records are applied to the owner's
-    bookkeeping, and host events that only the owner can resolve are combined over the ranks."""
+    """The ranks of a sharded ready set as contexts of this process; rank r owns the GLOBAL handles [cuts[r], cuts[r + 1])
+    (a range may be empty).  The host half follows ShardedScheduler: every rank declares every priority, the prefill mask
+    and the live level vectors are OR-ed over the ranks, records are applied to the owner's bookkeeping, host events that
+    only the owner can resolve are combined over the ranks, and worker state (free vectors, termination, min-utilisation,
+    the blocked mask) is replicated.  Its task calls are GpuScheduler's, with global handles, so that a drain
+    (tests/drain_fuzz.py) can drive it like a single context.  `make(flags)`, if given, returns a configured GpuScheduler
+    of one rank; otherwise every rank gets the classes and the prefill configuration given here."""
 
-    def __init__(self, R, classes, cuts, prefill, fused, prefill_of_rank=None):
+    levels_pruned_at = 0              # declared table size after the last pruning (the same on every rank)
+
+    def __init__(self, R, classes, cuts, prefill, fused, prefill_of_rank=None, make=None, flags=0):
         from hyperqueue_b200 import _lib as L
         self.L, self.fused = L, fused
-        flags = L.HQS_CREATE_SHARE_DEVICE if fused else 0
+        flags |= L.HQS_CREATE_SHARE_DEVICE if fused else 0
         self.parts = []
         for r, (lo, hi) in enumerate(zip(cuts[:-1], cuts[1:])):
             pf = prefill if prefill_of_rank is None else prefill_of_rank[r]
-            self.parts.append((_sched(R, classes, flags, pf), lo, hi))
+            self.parts.append((make(flags) if make else _sched(R, classes, flags, pf), lo, hi))
         if fused:
             n = len(self.parts)
             xb = (C.c_void_p * n)()
@@ -65,15 +71,27 @@ class Ranks:
         for s, _, _ in self.parts:
             s.new_worker(wid, res)
 
-    def add(self, handles, cls, prio):
+    def add_ready_tasks(self, handles, cls, prio):
         L = self.L
         h = np.asarray(handles, dtype=np.int64)
         lv = np.ascontiguousarray(np.unique(np.asarray(prio, dtype=np.uint64)))
         for s, lo, hi in self.parts:
+            s._sync_classes()
             s._check(s._lib.hqs_levels_add(s._ctx, lv.size, L.ptr(lv)))
             m = (h >= lo) & (h < hi)
             if m.any():
                 s.add_ready_tasks((h[m] - lo).astype(np.uint32), np.asarray(cls)[m], np.asarray(prio, dtype=np.uint64)[m])
+
+    add = add_ready_tasks             # the name the replays of this module and its importers call
+
+    def remove_ready_tasks(self, handles):
+        for s, _, mine in self._mine(handles):
+            if mine.size:
+                s.remove_ready_tasks(mine.astype(np.uint32))
+
+    def set_blocked_mask(self, mask):
+        for s, _, _ in self.parts:
+            s.set_blocked_mask(mask)
 
     def _mine(self, handles):
         h = np.asarray(handles, dtype=np.int64).reshape(-1)
@@ -92,8 +110,8 @@ class Ranks:
 
     def on_task_running_prefilled(self, t, variant):
         (s, lo, _), = [(s, lo, hi) for s, lo, hi in self.parts if lo <= t < hi]
-        pos = s._start_prefilled(t - lo, variant)
-        cls = int(s._task_class[t - lo])
+        pos = s._start_prefilled(int(t) - lo, variant)
+        cls = int(s._task_class[int(t) - lo])
         for s2, _, _ in self.parts:
             s2._take_resources(pos, cls, variant)
 
@@ -118,17 +136,37 @@ class Ranks:
             pf[lo:lo + m] = s._pf_worker[:m]
         return pf
 
-    def tick(self):
-        """One sharded tick on every rank.  Returns ([records of rank r, global handles], [free after], [(rc, text)])."""
+    def prune_levels(self):
+        """ShardedScheduler.prune_levels over the ranks: the same trigger, the OR of the live vectors, the same retain."""
+        from hyperqueue_b200.sharded import levels_need_pruning
+        s0 = self.parts[0][0]
+        if not levels_need_pruning(s0.n_declared_levels(), s0.n_classes, s0._prefill[1] > 0, self.levels_pruned_at):
+            return
+        tables = [s.levels_live() for s, _, _ in self.parts]
+        assert all(np.array_equal(lv, tables[0][0]) for lv, _ in tables)      # declared tables are identical
+        lives = [live for _, live in tables]
+        keep = np.bitwise_or.reduce(np.stack(lives), axis=0)
+        for s, _, _ in self.parts:
+            s.levels_retain(keep)
+        self.levels_pruned_at = int(np.count_nonzero(keep))
+
+    def tick(self, now=0.0):
+        """One sharded tick on every rank at time `now`.  Returns ([records of rank r, global handles], [free after],
+        [(rc, text)])."""
         from hyperqueue_b200.scheduler import apply_tick_records
         L = self.L
         s0 = self.parts[0][0]
         for s, _, _ in self.parts:
             s._sync_classes()
             assert np.array_equal(s.free, s0.free)            # the worker state is replicated
-        w = s0._worker_structs(0.0)
-        nw = w.shape[0]
-        free, total = np.ascontiguousarray(s0.free), np.ascontiguousarray(s0.total)
+        self.prune_levels()
+        # every rank passes its own copy of the replicated worker state, as a process of ShardedScheduler does
+        ins = []
+        for s, _, _ in self.parts:
+            blocked = s._blocked_bytes()
+            ins.append((s._worker_structs(now), np.ascontiguousarray(s.free), np.ascontiguousarray(s.total), blocked,
+                        L.ptr(blocked) if blocked is not None else None))
+        nw = ins[0][0].shape[0]
         masks = [s.prefill_mask() for s, _, _ in self.parts if s._prefill[1] > 0]
         if masks:
             mask = np.ascontiguousarray(np.bitwise_or.reduce(np.stack(masks), axis=0))
@@ -138,16 +176,16 @@ class Ranks:
         caps = [max(hi - lo, 1) for _, lo, hi in self.parts]
         if self.fused:
             # the ticks wait for each other on the device: every buffer is allocated before the first launch
-            for (s, _, _), cap in zip(self.parts, caps):
-                s._check(s._lib.hqs_tick_reserve(s._ctx, nw, cap, 0))
-            for (s, _, _), cap in zip(self.parts, caps):
-                s._check(s._lib.hqs_shard_tick_launch(s._ctx, nw, L.ptr(w), L.ptr(free), L.ptr(total), None, cap))
+            for (s, _, _), cap, (_, _, _, blocked, _) in zip(self.parts, caps, ins):
+                s._check(s._lib.hqs_tick_reserve(s._ctx, nw, cap, int(blocked is not None)))
+            for (s, _, _), cap, (w, free, total, _, bp) in zip(self.parts, caps, ins):
+                s._check(s._lib.hqs_shard_tick_launch(s._ctx, nw, L.ptr(w), L.ptr(free), L.ptr(total), bp, cap))
         else:
             counts = []
-            for s, _, _ in self.parts:
+            for (s, _, _), (w, free, total, _, bp) in zip(self.parts, ins):
                 c = torch.zeros(L.HQS_MAX_GROUPS, dtype=torch.int32, device="cuda")
                 ng = C.c_uint32(0)
-                s._check(s._lib.hqs_shard_count(s._ctx, nw, L.ptr(w), L.ptr(free), L.ptr(total), None,
+                s._check(s._lib.hqs_shard_count(s._ctx, nw, L.ptr(w), L.ptr(free), L.ptr(total), bp,
                                                 C.c_void_p(c.data_ptr()), c.numel(), C.byref(ng)))
                 counts.append(c)
             st = torch.stack(counts).to(torch.int64)
@@ -160,7 +198,7 @@ class Ranks:
                 s._check(s._lib.hqs_shard_solve_emit(s._ctx, C.c_void_p(all_c.data_ptr()), C.c_void_p(befs[r].data_ptr()), cap))
             out = np.zeros(cap, dtype=L.assignment_dtype)
             n = C.c_uint32(0)
-            fa = np.zeros_like(free)
+            fa = np.zeros_like(s.free)
             rc = s._lib.hqs_tick_fetch(s._ctx, cap, L.ptr(out), C.byref(n), L.ptr(fa))
             errs.append((rc, (s._lib.hqs_last_error(s._ctx) or b"").decode() if rc else ""))
             a = out[: n.value].copy()

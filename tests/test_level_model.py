@@ -147,3 +147,53 @@ def test_coarse_pushes_register_their_priorities():
     m.classes_set(3)
     assert m.coarsened == 0 and m.n_levels == 1500
     _check_invariants(m, False)
+
+
+def test_levels_live_and_retain():
+    """Declared levels: live flags follow the VALID keys; a retain that drops a carried level or has another length is
+    rejected with nothing changed; a valid one drops the dead levels, leaves coarse mode when the rest fits, re-levels."""
+    m = LM.LevelModel()
+    m.classes_set(4096)                                   # budget 2 levels
+    m.levels_add([50, 40, 30, 20])
+    assert m.coarsened == 1
+    m.push([0, 1, 2], [0, 1, 2], [40, 20, 40])
+    lv, live = m.levels_live()
+    assert lv.tolist() == [50, 40, 30, 20] and live.tolist() == [0, 1, 0, 1]
+    keys = m.keys().copy()
+    for bad in ([1, 0, 1, 1], [0, 1, 0, 1, 1], [0, 1, 0]):
+        with pytest.raises(LM.Rejected):
+            m.levels_retain(bad)
+        assert np.array_equal(m.keys(), keys) and m.levels == [50, 40, 30, 20]
+    m.levels_retain([1, 1, 0, 1])                          # another rank still holds 50
+    assert m.levels == [50, 40, 20] and m.coarsened == 1 and m.pruned_at == 3
+    m.remove([0, 2])
+    m.levels_retain(m.levels_live()[1])
+    assert m.levels == [20] and m.coarsened == 0 and m.pruned_at == 1
+    assert int(m.lvl[1]) == 0 and not m.need_pruning()    # declared: never prunes on its own
+
+
+def test_random_declared_sequences_retain_levels():
+    rng = np.random.default_rng(3)
+    m = LM.LevelModel()
+    m.classes_set(2)
+    used: set = set()
+    kinds = {}
+    for _ in range(400):
+        op = LM.random_op(rng, m, used, declared=True)
+        kinds[op[0]] = kinds.get(op[0], 0) + 1
+        try:
+            if op[0] == "push":
+                m.push(op[1], op[2], op[3])
+            elif op[0] == "remove":
+                m.remove(op[1])
+            elif op[0] == "levels_add":
+                m.levels_add(op[1])
+            elif op[0] == "levels_retain":
+                m.levels_retain(op[1])
+            elif op[0] == "classes":
+                m.classes_set(op[1])
+        except LM.Rejected:
+            continue
+        # every carried priority stays registered
+        assert set(int(p) for p in m.live_priorities().tolist()) <= set(m.levels)
+    assert kinds.get("levels_retain", 0) > 5, kinds

@@ -181,3 +181,66 @@ def test_sharded_tasks_finished_returns_resources_on_every_rank():
     total = np.full((3, 2), 80000, dtype=np.uint64)
     for rank in range(world):
         assert np.array_equal(np.frombuffer(ret[rank], dtype=np.uint64).reshape(3, 2), total)
+
+
+def _mirror_with_unlimited(n_local, W, R):
+    """_FakeMirror with resource 1 of worker 2 unlimited (HQS_AMOUNT_MAX), and the fields the record bookkeeping reads."""
+    from hyperqueue_b200 import _lib as L
+    s = _FakeMirror(n_local, W, R)
+    s.worker_ids = np.arange(W, dtype=np.uint32)
+    s._pf_worker = np.full(n_local, -1, dtype=np.int64)
+    s.total[2, 1] = L.HQS_AMOUNT_MAX
+    s.free = s.total.copy()
+    return s
+
+
+def _finish_on_unlimited(rank, world):
+    """Global task t of class t % 2 ran on worker t % 3; task 5 requested resource 1 of worker 2, whose total is
+    HQS_AMOUNT_MAX (a tick leaves it unlimited).  All tasks finish; returns the rank's free vectors afterwards."""
+    from hyperqueue_b200 import _lib as L
+    from hyperqueue_b200.sharded import ShardedScheduler, block_range
+    n_total, W, R = 10, 3, 2
+    lo, hi = block_range(n_total, rank, world)
+    sh = ShardedScheduler.__new__(ShardedScheduler)
+    sh.s, sh.rank, sh.world, sh.group, sh.lo, sh.hi, sh.device = (_mirror_with_unlimited(hi - lo, W, R), rank, world, None,
+                                                                   lo, hi, torch.device("cpu"))
+    for t in range(n_total):
+        fr = sh.s.free[t % 3]
+        sh.s.free[t % 3] = np.where(fr == np.uint64(L.HQS_AMOUNT_MAX), fr, fr - sh.s._amount_tab[t % 2, 0])
+    a = np.zeros(hi - lo, dtype=[("task", "<u4"), ("worker", "<u2"), ("variant", "u1"), ("kind", "u1")])
+    a["task"] = np.arange(hi - lo); a["worker"] = (np.arange(lo, hi) % 3)
+    sh.s._task_class[:] = np.arange(lo, hi) % 2
+    sh._record(a)
+    sh.tasks_finished(np.arange(n_total))
+    return sh.s.free
+
+
+def _unlimited_worker(rank, world, port, ret):
+    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
+    dist.init_process_group("gloo", rank=rank, world_size=world)
+    ret[rank] = _finish_on_unlimited(rank, world).tobytes()
+    dist.barrier()
+    dist.destroy_process_group()
+
+
+def _totals_with_unlimited():
+    from hyperqueue_b200 import _lib as L
+    total = np.full((3, 2), 80000, dtype=np.uint64)
+    total[2, 1] = L.HQS_AMOUNT_MAX
+    return total
+
+
+def test_sharded_tasks_finished_keeps_unlimited_amounts_in_a_world_of_one():
+    """A task that requested resource 1 finishes on the worker whose resource 1 is HQS_AMOUNT_MAX: it stays MAX (adding the
+    returned amount onto it would wrap to amount - 1)."""
+    assert np.array_equal(_finish_on_unlimited(0, 1), _totals_with_unlimited())
+
+
+def test_sharded_tasks_finished_keeps_unlimited_amounts_on_every_rank():
+    """The same over gloo with two ranks: the task on the unlimited worker belongs to rank 1, and both ranks keep MAX."""
+    world = 2
+    mgr = mp.Manager()
+    ret = mgr.dict()
+    mp.spawn(_unlimited_worker, args=(world, _free_port(), ret), nprocs=world, join=True)
+    for rank in range(world):
+        assert np.array_equal(np.frombuffer(ret[rank], dtype=np.uint64).reshape(3, 2), _totals_with_unlimited())

@@ -163,3 +163,35 @@ def test_prefill_mask_world_one_is_the_local_mask():
     from hyperqueue_b200.sharded import reduce_prefill_mask
     m = np.eye(4, 3, dtype=np.uint8)
     assert np.array_equal(reduce_prefill_mask(m, 1), m)
+
+
+def _live_worker(rank, world, port, ret):
+    """Per-rank live vectors of a declared level table: the OR is what every rank passes to hqs_levels_retain."""
+    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
+    dist.init_process_group("gloo", rank=rank, world_size=world)
+    from hyperqueue_b200.sharded import reduce_or
+    rng = np.random.default_rng(70 + rank)
+    live = (rng.random(300) < 0.05).astype(np.uint8)
+    ret[rank] = (live.tobytes(), reduce_or(live, world).tobytes())
+    dist.barrier()
+    dist.destroy_process_group()
+
+
+def test_level_live_vectors_are_or_ed_over_the_ranks():
+    world = 2
+    mgr = mp.Manager()
+    ret = mgr.dict()
+    mp.spawn(_live_worker, args=(world, _free_port(), ret), nprocs=world, join=True)
+    lives = [np.frombuffer(ret[r][0], dtype=np.uint8) for r in range(world)]
+    want = lives[0] | lives[1]
+    assert (lives[0] & ~lives[1]).any() and (lives[1] & ~lives[0]).any()        # each rank alone would drop a live level
+    for r in range(world):
+        assert np.array_equal(np.frombuffer(ret[r][1], dtype=np.uint8), want)
+
+
+def test_levels_need_pruning_budget_and_doubling():
+    from hyperqueue_b200.sharded import levels_need_pruning
+    assert not levels_need_pruning(256, 16, True, 200) and levels_need_pruning(257, 16, True, 200)      # 8192 / (2 * 16)
+    assert not levels_need_pruning(512, 16, False, 300) and levels_need_pruning(513, 16, False, 300)    # 8192 / 16
+    assert not levels_need_pruning(128, 64, False, 32) and levels_need_pruning(129, 64, False, 100)
+    assert not levels_need_pruning(84, 2, False, 10) and levels_need_pruning(85, 2, False, 10)          # 2 * 10 + 64
