@@ -1,0 +1,254 @@
+// hqs_graph.cuh — task graphs that grow while the ready set runs: hqs_graph_push / hqs_graph_finished (on_new_tasks and
+// task_finished, reactor.rs:188-220, 500-580).  Included by hqsched.cu inside its anonymous namespace, after
+// hqs_ready_set.cuh.
+//
+// Per handle h (allocated at the first graph push, grown with the task table):
+//   gdeps[h]  u32  unfinished counted dependencies of h's current incarnation
+//   ggen[h]   u32  incarnation: +1 at every hqs_graph_push of h
+//   ghead[h]  u32  first edge of h's consumer list, GRAPH_NIL = none
+// Edge pool: GraphEdge {consumer, consumer's incarnation, next}.  A push takes its slots by the batch's dependency offsets
+// (no atomics) and links each counted edge in front of its producer's list.  A list is emptied whenever its producer
+// leaves the table (finished or removed), so head[h] != GRAPH_NIL implies that h is VALID.
+#pragma once
+
+constexpr u32 GRAPH_NIL = ~0u;
+constexpr u32 GRAPH_POOL_MIN = 4096;      // edge slots of a fresh pool
+constexpr u32 GRAPH_NT = 256;             // threads of the counting / emitting kernels
+constexpr u32 GRAPH_PER_THREAD = 8;       // consecutive words (ready bitmap) or handles (pool compaction) per thread
+constexpr u32 GRAPH_PER_BLOCK = GRAPH_NT * GRAPH_PER_THREAD;
+
+struct GraphEdge {
+    u32 cons;   // consumer handle
+    u32 gen;    // the consumer's incarnation the edge was made for
+    u32 next;   // next edge of the producer's list
+};
+
+// exclusive prefix sum over the block (NT <= 1024); *total receives the block's sum in every thread
+template <u32 NT>
+__device__ __forceinline__ u32 graph_block_scan(u32 v, u32* total) {
+    __shared__ u32 warp_off[NT / 32];
+    __shared__ u32 block_sum;
+    const u32 lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    u32 x = v;
+    for (u32 o = 1; o < 32; o <<= 1) {
+        const u32 y = __shfl_up_sync(0xffffffffu, x, o);
+        if (lane >= o) x += y;
+    }
+    if (lane == 31) warp_off[wid] = x;
+    __syncthreads();
+    if (wid == 0) {
+        const u32 s = lane < NT / 32 ? warp_off[lane] : 0u;
+        u32 t = s;
+        for (u32 o = 1; o < 32; o <<= 1) {
+            const u32 y = __shfl_up_sync(0xffffffffu, t, o);
+            if (lane >= o) t += y;
+        }
+        if (lane < NT / 32) warp_off[lane] = t - s;
+        if (lane == 31) block_sum = t;
+    }
+    __syncthreads();
+    const u32 r = warp_off[wid] + x - v;
+    *total = block_sum;
+    __syncthreads();   // the shared words may be reused by the next call
+    return r;
+}
+
+// single block: in-place exclusive scan of nb per-block sums; *total = their sum
+__global__ void __launch_bounds__(1024) graph_scan_k(u32 nb, u32* __restrict__ blk, u32* __restrict__ total) {
+    u32 carry = 0;
+    for (u32 base = 0; base < nb; base += 1024) {
+        const u32 i = base + threadIdx.x;
+        const u32 v = i < nb ? blk[i] : 0u;
+        u32 sum;
+        const u32 ex = graph_block_scan<1024>(v, &sum);
+        if (i < nb) blk[i] = carry + ex;
+        carry += sum;
+    }
+    if (threadIdx.x == 0) *total = carry;
+}
+
+// a pushed handle that is still VALID rejects the batch (flag[1] bit 1; push_k and graph_link_k then write nothing).
+// Handles >= n_handles have never been pushed.
+__global__ void graph_validate_k(u32 n, const u32* __restrict__ task, const u32* __restrict__ key, u32 n_handles,
+                                 u32* __restrict__ flag) {
+    const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
+    const u32 h = i < n ? task[i] : GRAPH_NIL;
+    const bool bad = h < n_handles && (key[h] & KEY_VALID);
+    if (__ballot_sync(0xffffffffu, bad) && (threadIdx.x & 31) == 0) atomicOr(&flag[1], 2u);
+}
+
+// after push_k: task i's dependencies are dep[off[i] .. off[i+1]) (the host dropped those on later tasks of the batch).  One
+// counts if its producer is VALID: a task of the table or an earlier task of the batch (push_k made those VALID).  Counted
+// edges take slot e0 + j and are linked into the producer's list; a task with a counted dependency is waiting (READY
+// cleared).  n_ready[0] += tasks ready at once.
+__global__ void graph_link_k(u32 n, const u32* __restrict__ task, const u32* __restrict__ off, const u32* __restrict__ dep,
+                             u32 e0, const u32* __restrict__ flag, u32* key, u32* __restrict__ gdeps,
+                             u32* __restrict__ ggen, u32* __restrict__ ghead, GraphEdge* __restrict__ pool,
+                             u32* __restrict__ n_ready) {
+    if (flag[1]) return;                    // the batch was rejected
+    const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
+    bool ready = false;
+    if (i < n) {
+        const u32 h = task[i];
+        const u32 g = ggen[h] + 1;
+        ggen[h] = g;
+        u32 cnt = 0;
+        for (u32 j = off[i], hi = off[i + 1]; j < hi; ++j) {
+            const u32 p = dep[j];
+            if (!(key[p] & KEY_VALID)) continue;            // finished, removed or never pushed: dropped
+            const u32 e = e0 + j;
+            pool[e].cons = h;
+            pool[e].gen = g;
+            pool[e].next = atomicExch(&ghead[p], e);
+            ++cnt;
+        }
+        gdeps[h] = cnt;
+        if (cnt) key[h] &= ~KEY_READY;      // only this thread writes key[h]; the others read its VALID bit
+        ready = cnt == 0;
+    }
+    const u32 made = __popc(__ballot_sync(0xffffffffu, ready));
+    if ((threadIdx.x & 31) == 0 && made) atomicAdd(n_ready, made);
+}
+
+// hqs_graph_finished, phase 1: every finished task leaves the table.  Only the thread that clears VALID keeps the handle
+// (win[i]), so a handle named twice, or one that is not VALID, walks no list.  All tasks of the batch have left before any
+// consumer is looked at (phase 2), so a consumer finished in the same batch is never released.
+__global__ void graph_leave_k(u32 n, const u32* __restrict__ task, u32* __restrict__ key, u32* __restrict__ win) {
+    const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const u32 h = task[i];
+    const u32 old = atomicAnd(&key[h], ~(KEY_READY | KEY_VALID | KEY_DONE | KEY_PF));
+    win[i] = (old & KEY_VALID) ? h : GRAPH_NIL;
+}
+
+// the consumer of edge E still waits on the incarnation E was made for
+__device__ __forceinline__ bool graph_edge_waits(const GraphEdge& E, const u32* key, const u32* __restrict__ ggen) {
+    return ggen[E.cons] == E.gen && (key[E.cons] & (KEY_VALID | KEY_READY | KEY_DONE)) == KEY_VALID;
+}
+
+// phase 2: each kept handle walks its consumers; the decrement that reaches zero makes the consumer READY and flags it in the
+// ready bitmap (one bit per handle).  Then the list is emptied.
+__global__ void graph_release_k(u32 n, const u32* __restrict__ win, u32* key, u32* __restrict__ gdeps,
+                                const u32* __restrict__ ggen, u32* __restrict__ ghead, const GraphEdge* __restrict__ pool,
+                                u32* __restrict__ bits) {
+    const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const u32 h = win[i];
+    if (h == GRAPH_NIL) return;
+    for (u32 e = ghead[h]; e != GRAPH_NIL;) {
+        const GraphEdge E = pool[e];
+        if (graph_edge_waits(E, key, ggen) && atomicSub(&gdeps[E.cons], 1u) == 1u) {
+            atomicOr(&key[E.cons], KEY_READY);
+            atomicOr(&bits[E.cons >> 5], 1u << (E.cons & 31));
+        }
+        e = E.next;
+    }
+    ghead[h] = GRAPH_NIL;
+}
+
+// phase 3: ordered compaction of the ready bitmap.  Thread t of block b owns the words [(b * NT + t) * 8, + 8).
+__global__ void __launch_bounds__(GRAPH_NT) graph_ready_count_k(u32 n_words, const u32* __restrict__ bits,
+                                                                 u32* __restrict__ blk) {
+    const u32 w0 = (blockIdx.x * GRAPH_NT + threadIdx.x) * GRAPH_PER_THREAD;
+    u32 c = 0;
+#pragma unroll
+    for (u32 k = 0; k < GRAPH_PER_THREAD; ++k)
+        if (w0 + k < n_words) c += __popc(bits[w0 + k]);
+    u32 sum;
+    graph_block_scan<GRAPH_NT>(c, &sum);
+    if (threadIdx.x == 0) blk[blockIdx.x] = sum;
+}
+
+// blk = exclusive scan of graph_ready_count_k's sums: the handles come out ascending, and the bitmap is cleared
+__global__ void __launch_bounds__(GRAPH_NT) graph_ready_emit_k(u32 n_words, u32* __restrict__ bits,
+                                                                const u32* __restrict__ blk, u32* __restrict__ out) {
+    const u32 w0 = (blockIdx.x * GRAPH_NT + threadIdx.x) * GRAPH_PER_THREAD;
+    u32 w[GRAPH_PER_THREAD];
+    u32 c = 0;
+#pragma unroll
+    for (u32 k = 0; k < GRAPH_PER_THREAD; ++k) {
+        w[k] = w0 + k < n_words ? bits[w0 + k] : 0u;
+        c += __popc(w[k]);
+    }
+    u32 sum;
+    u32 pos = blk[blockIdx.x] + graph_block_scan<GRAPH_NT>(c, &sum);
+#pragma unroll
+    for (u32 k = 0; k < GRAPH_PER_THREAD; ++k) {
+        u32 x = w[k];
+        if (!x) continue;
+        bits[w0 + k] = 0u;
+        while (x) {
+            out[pos++] = (w0 + k) * 32u + (u32)(__ffs(x) - 1);
+            x &= x - 1;
+        }
+    }
+}
+
+// hqs_ready_remove on a graph context: the removed producers' lists are emptied (their consumers stay waiting)
+__global__ void graph_unlink_k(u32 n, const u32* __restrict__ task, u32 n_handles, u32* __restrict__ ghead) {
+    const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const u32 h = task[i];
+    if (h < n_handles) ghead[h] = GRAPH_NIL;
+}
+
+// pool compaction, pass 1: edges whose consumer still waits on their incarnation, per block of 2048 producers
+__global__ void __launch_bounds__(GRAPH_NT) graph_gc_count_k(u32 n_handles, const u32* __restrict__ ghead,
+                                                              const GraphEdge* __restrict__ pool, const u32* __restrict__ key,
+                                                              const u32* __restrict__ ggen, u32* __restrict__ blk) {
+    const u32 h0 = (blockIdx.x * GRAPH_NT + threadIdx.x) * GRAPH_PER_THREAD;
+    u32 c = 0;
+    for (u32 k = 0; k < GRAPH_PER_THREAD; ++k) {
+        if (h0 + k >= n_handles) break;
+        for (u32 e = ghead[h0 + k]; e != GRAPH_NIL; e = pool[e].next) c += graph_edge_waits(pool[e], key, ggen) ? 1u : 0u;
+    }
+    u32 sum;
+    graph_block_scan<GRAPH_NT>(c, &sum);
+    if (threadIdx.x == 0) blk[blockIdx.x] = sum;
+}
+
+// pass 2 (blk scanned): every list is rewritten, in its order, into consecutive slots of the fresh pool
+__global__ void __launch_bounds__(GRAPH_NT) graph_gc_move_k(u32 n_handles, u32* __restrict__ ghead,
+                                                             const GraphEdge* __restrict__ pool, GraphEdge* __restrict__ fresh,
+                                                             const u32* __restrict__ key, const u32* __restrict__ ggen,
+                                                             const u32* __restrict__ blk) {
+    const u32 h0 = (blockIdx.x * GRAPH_NT + threadIdx.x) * GRAPH_PER_THREAD;
+    u32 c = 0;
+    for (u32 k = 0; k < GRAPH_PER_THREAD; ++k) {
+        if (h0 + k >= n_handles) break;
+        for (u32 e = ghead[h0 + k]; e != GRAPH_NIL; e = pool[e].next) c += graph_edge_waits(pool[e], key, ggen) ? 1u : 0u;
+    }
+    u32 sum;
+    u32 pos = blk[blockIdx.x] + graph_block_scan<GRAPH_NT>(c, &sum);
+    for (u32 k = 0; k < GRAPH_PER_THREAD; ++k) {
+        const u32 h = h0 + k;
+        if (h >= n_handles) break;
+        u32 first = GRAPH_NIL, prev = GRAPH_NIL;
+        for (u32 e = ghead[h]; e != GRAPH_NIL; e = pool[e].next) {
+            const GraphEdge E = pool[e];
+            if (!graph_edge_waits(E, key, ggen)) continue;
+            fresh[pos] = GraphEdge{E.cons, E.gen, GRAPH_NIL};
+            if (prev == GRAPH_NIL) first = pos; else fresh[prev].next = pos;
+            prev = pos++;
+        }
+        ghead[h] = first;
+    }
+}
+
+// hqs_graph_debug: out[0] += linked edges, out[1] += waiting tasks (VALID, neither READY nor DONE)
+__global__ void graph_debug_k(u32 n_handles, const u32* __restrict__ key, const u32* __restrict__ ghead,
+                              const GraphEdge* __restrict__ pool, unsigned long long* __restrict__ out) {
+    const u32 h = blockIdx.x * blockDim.x + threadIdx.x;
+    u32 edges = 0, waiting = 0;
+    if (h < n_handles) {
+        if (ghead)
+            for (u32 e = ghead[h]; e != GRAPH_NIL; e = pool[e].next) ++edges;
+        waiting = (key[h] & (KEY_VALID | KEY_READY | KEY_DONE)) == KEY_VALID ? 1u : 0u;
+    }
+    edges = __reduce_add_sync(0xffffffffu, edges);
+    waiting = __reduce_add_sync(0xffffffffu, waiting);
+    if ((threadIdx.x & 31) == 0) {
+        if (edges) atomicAdd(&out[0], (unsigned long long)edges);
+        if (waiting) atomicAdd(&out[1], (unsigned long long)waiting);
+    }
+}

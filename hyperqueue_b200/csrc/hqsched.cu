@@ -15,6 +15,7 @@
 //   key[h]   u32  bit31 READY | bit30 DONE (assigned by a tick) | bit29 VALID | bit28 PREFILLED | level(14) | class(14)
 //   prio[h]  u64  tako Priority (only read when the level table changes)
 //   deps[h]  u32  unfinished dependencies (DAG mode), cons_off/cons: CSR of consumers
+//   gdeps[h], ggen[h], ghead[h] + an edge pool: task graphs grown by hqs_graph_push (hqs_graph.cuh)
 // One tick = ONE cooperative kernel (tick_k, hqs_tick.cuh):
 //   worker CTAs : per-chunk histogram of ready tasks by group g = level*Q + class (HBM streaming, 4 B/task), exclusive
 //                 scan of the chunk table over chunks, on request the pack step (one warp fills one worker), then the
@@ -52,6 +53,7 @@ typedef uint32_t u32;
 typedef uint64_t u64;
 
 #include "hqs_ready_set.cuh"
+#include "hqs_graph.cuh"
 #include "hqs_solver.cuh"
 #include "hqs_tick.cuh"
 #include "hqs_group.cuh"
@@ -111,6 +113,21 @@ struct hqs_ctx {
     u32* d_cons_off = nullptr;
     u32* d_cons = nullptr;
     bool dag = false;
+    // task graph (hqs_graph_push / hqs_graph_finished, hqs_graph.cuh): nothing of it exists before the first graph call
+    bool graph_storage = false;         // the per-handle arrays below exist and grow with the table
+    bool graph = false;                 // a graph push was accepted: hqs_dag_load is refused
+    u32* d_gdeps = nullptr; u32* d_ggen = nullptr; u32* d_ghead = nullptr;
+    u32* d_gbits = nullptr;             // [cap_handles / 32] ready bitmap of hqs_graph_finished (zero between calls)
+    u32* d_gready = nullptr;            // [cap_handles] the newly ready handles, ascending
+    u32* d_gblk = nullptr;              // [cap_handles / GRAPH_PER_BLOCK + 1] per-block sums of the ordered compactions
+    u32* d_gsmall = nullptr;            // [4] n_ready of a push, n_new of a finish, live edges of a compaction
+    GraphEdge* d_pool = nullptr;
+    u32 pool_cap = 0, pool_used = 0;    // edge slots; slots [0, pool_used) have been handed out since the last compaction
+    u64 pool_compactions = 0;
+    u32* d_gstage = nullptr; size_t gstage_cap = 0;   // a push's dependency offsets [n + 1] and dependencies
+    std::vector<u32> g_off, g_dep;      // host scratch of hqs_graph_push
+    std::vector<std::pair<u32, u32>> g_pos;
+    std::vector<u32> g_new_ready;       // what *new_ready of hqs_graph_finished points to
     // push staging (device)
     u32* d_push_task = nullptr; u32* d_push_cls = nullptr; u64* d_push_prio = nullptr;
     u32 push_cap = 0;
@@ -207,7 +224,45 @@ int ensure_handles(hqs_ctx* ctx, u32 need) {
     int rc;
     if ((rc = dev_realloc(ctx, &ctx->d_key, ctx->cap_handles, cap, true, true))) return rc;
     if ((rc = dev_realloc(ctx, &ctx->d_prio, ctx->cap_handles, cap, true, true))) return rc;
+    if (ctx->graph_storage) {
+        if ((rc = dev_realloc(ctx, &ctx->d_gdeps, ctx->cap_handles, cap, true, true))) return rc;
+        if ((rc = dev_realloc(ctx, &ctx->d_ggen, ctx->cap_handles, cap, true, true))) return rc;
+        if ((rc = dev_realloc(ctx, &ctx->d_ghead, ctx->cap_handles, cap, true, false))) return rc;
+        CU(cudaMemsetAsync(ctx->d_ghead + ctx->cap_handles, 0xFF, (size_t)(cap - ctx->cap_handles) * 4, ctx->stream));
+        if ((rc = dev_realloc(ctx, &ctx->d_gbits, ctx->cap_handles / 32, cap / 32, true, true))) return rc;
+        if ((rc = dev_realloc(ctx, &ctx->d_gready, 0, cap, false, false))) return rc;
+        if ((rc = dev_realloc(ctx, &ctx->d_gblk, 0, cap / GRAPH_PER_BLOCK + 1, false, false))) return rc;
+    }
     ctx->cap_handles = cap;
+    return HQS_OK;
+}
+
+// the per-handle graph arrays, at the table's current capacity (ensure_handles grows them from then on)
+int ensure_graph_storage(hqs_ctx* ctx) {
+    if (ctx->graph_storage) return HQS_OK;
+    const u32 cap = ctx->cap_handles;
+    int rc;
+    if (!ctx->d_gsmall) CU(cudaMalloc(&ctx->d_gsmall, 4 * sizeof(u32)));
+    if ((rc = dev_realloc(ctx, &ctx->d_gdeps, 0, cap, false, true))) return rc;
+    if ((rc = dev_realloc(ctx, &ctx->d_ggen, 0, cap, false, true))) return rc;
+    if ((rc = dev_realloc(ctx, &ctx->d_ghead, 0, cap, false, false))) return rc;
+    CU(cudaMemsetAsync(ctx->d_ghead, 0xFF, (size_t)cap * 4, ctx->stream));
+    if ((rc = dev_realloc(ctx, &ctx->d_gbits, 0, cap / 32, false, true))) return rc;
+    if ((rc = dev_realloc(ctx, &ctx->d_gready, 0, cap, false, false))) return rc;
+    if ((rc = dev_realloc(ctx, &ctx->d_gblk, 0, cap / GRAPH_PER_BLOCK + 1, false, false))) return rc;
+    ctx->graph_storage = true;
+    return HQS_OK;
+}
+
+// device staging of a batch's handles (and class ids / priorities) for the ready-set calls
+int ensure_push_staging(hqs_ctx* ctx, u32 n) {
+    if (n <= ctx->push_cap) return HQS_OK;
+    CU(cudaStreamSynchronize(ctx->stream));
+    if (ctx->d_push_task) { CU(cudaFree(ctx->d_push_task)); CU(cudaFree(ctx->d_push_cls)); CU(cudaFree(ctx->d_push_prio)); }
+    ctx->push_cap = std::max<u32>(n, 1u << 16);
+    CU(cudaMalloc(&ctx->d_push_task, (size_t)ctx->push_cap * 4));
+    CU(cudaMalloc(&ctx->d_push_cls, (size_t)ctx->push_cap * 4));
+    CU(cudaMalloc(&ctx->d_push_prio, (size_t)ctx->push_cap * 8));
     return HQS_OK;
 }
 
@@ -976,7 +1031,9 @@ void hqs_destroy(hqs_ctx* ctx) {
                         ctx->d_cons, ctx->d_push_task, ctx->d_push_cls, ctx->d_push_prio, ctx->d_newcnt,
                         ctx->d_newprio, ctx->d_table, ctx->d_total, ctx->d_gout, ctx->d_rem_scratch, ctx->d_excl, ctx->d_gout2, ctx->d_pf_cum, ctx->d_pf_wk, ctx->d_seg_cum,
                         ctx->d_seg_wv, ctx->d_out, ctx->d_hdr, ctx->d_free_after, ctx->d_tickin, ctx->d_sync, ctx->d_pk_fr,
-                        ctx->d_pk_quota, ctx->d_pk_taken, ctx->d_pk_cand, ctx->d_pk_meta, ctx->d_prune_lv, ctx->d_prune_live};
+                        ctx->d_pk_quota, ctx->d_pk_taken, ctx->d_pk_cand, ctx->d_pk_meta, ctx->d_prune_lv, ctx->d_prune_live,
+                        ctx->d_gdeps, ctx->d_ggen, ctx->d_ghead, ctx->d_gbits, ctx->d_gready, ctx->d_gblk, ctx->d_gsmall,
+                        ctx->d_pool, ctx->d_gstage};
     for (void* p : dev_ptrs) if (p) cudaFree(p);
     for (void* p : ctx->x_opened) cudaIpcCloseMemHandle(p);
     if (ctx->d_xbuf) cudaFree(ctx->d_xbuf);
@@ -1087,19 +1144,21 @@ int hqs_classes_set(hqs_ctx* ctx, uint32_t n_classes, const hqs_class* classes) 
 }
 
 namespace {
-// shared body of hqs_ready_push / hqs_ready_push_range (task == nullptr: handles first_handle .. first_handle + n - 1)
-int push_impl(hqs_ctx* ctx, u32 n, const u32* task, u32 first_handle, const u32* class_id, const u64* priority) {
+// The dependencies of a graph push, staged by hqs_graph_push: d_gstage = dependency offsets [n + 1], then the dependency
+// handles; the counted edges take the pool slots e0 + j.
+struct GraphBatch {
+    u32 e0;
+};
+
+// shared body of hqs_ready_push / hqs_ready_push_range (task == nullptr: handles first_handle .. first_handle + n - 1) and
+// hqs_graph_push (g != nullptr: the batch is also rejected if a pushed handle is VALID, and graph_link_k runs after push_k;
+// h_small[2] receives the number of tasks ready at once)
+int push_impl(hqs_ctx* ctx, u32 n, const u32* task, u32 first_handle, const u32* class_id, const u64* priority,
+              const GraphBatch* g = nullptr) {
     if (ctx->Q == 0) return fail(ctx, HQS_E_STATE, "hqs_classes_set has not been called");
     if (ctx->dag) return fail(ctx, HQS_E_STATE, "hqs_ready_push is not available after hqs_dag_load");
     CU(cudaSetDevice(ctx->device));
-    if (n > ctx->push_cap) {
-        CU(cudaStreamSynchronize(ctx->stream));
-        if (ctx->d_push_task) { CU(cudaFree(ctx->d_push_task)); CU(cudaFree(ctx->d_push_cls)); CU(cudaFree(ctx->d_push_prio)); }
-        ctx->push_cap = std::max<u32>(n, 1u << 16);
-        CU(cudaMalloc(&ctx->d_push_task, (size_t)ctx->push_cap * 4));
-        CU(cudaMalloc(&ctx->d_push_cls, (size_t)ctx->push_cap * 4));
-        CU(cudaMalloc(&ctx->d_push_prio, (size_t)ctx->push_cap * 8));
-    }
+    if (int rc_ = ensure_push_staging(ctx, n)) return rc_;
     if (task) CU(cudaMemcpyAsync(ctx->d_push_task, task, (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream));
     CU(cudaMemcpyAsync(ctx->d_push_cls, class_id, (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream));
     CU(cudaMemcpyAsync(ctx->d_push_prio, priority, (size_t)n * 8, cudaMemcpyHostToDevice, ctx->stream));
@@ -1120,10 +1179,19 @@ int push_impl(hqs_ctx* ctx, u32 n, const u32* task, u32 first_handle, const u32*
     if (rc) { cudaStreamSynchronize(ctx->stream); return rc; }
     CU(cudaMemsetAsync(ctx->d_newcnt, 0, 2 * sizeof(u32), ctx->stream));
     push_validate_k<<<(n + 255) / 256, 256, 0, ctx->stream>>>(n, ctx->d_push_cls, ctx->Q, ctx->d_newcnt);
+    if (g) graph_validate_k<<<(n + 255) / 256, 256, 0, ctx->stream>>>(n, ctx->d_push_task, ctx->d_key, ctx->n_handles, ctx->d_newcnt);
     push_k<<<(n + 255) / 256, 256, 0, ctx->stream>>>(n, task ? ctx->d_push_task : nullptr, first_handle, ctx->d_push_cls,
                                                      ctx->d_push_prio, ctx->d_key, ctx->d_prio, ctx->d_levels,
                                                      (u32)ctx->dev_levels.size(), ctx->coarse ? 1 : 0, ctx->d_newcnt, ctx->d_newprio);
     ctx->stats.kernel_launches += 2;
+    if (g) {
+        CU(cudaMemsetAsync(ctx->d_gsmall, 0, sizeof(u32), ctx->stream));
+        graph_link_k<<<(n + 255) / 256, 256, 0, ctx->stream>>>(n, ctx->d_push_task, ctx->d_gstage, ctx->d_gstage + n + 1, g->e0,
+                                                               ctx->d_newcnt, ctx->d_key, ctx->d_gdeps, ctx->d_ggen, ctx->d_ghead,
+                                                               ctx->d_pool, ctx->d_gsmall);
+        CU(cudaMemcpyAsync(ctx->h_small + 2, ctx->d_gsmall, sizeof(u32), cudaMemcpyDeviceToHost, ctx->stream));
+        ctx->stats.kernel_launches += 2;
+    }
     CU(cudaGetLastError());
     CU(cudaMemcpyAsync(ctx->h_small, ctx->d_newcnt, 2 * sizeof(u32), cudaMemcpyDeviceToHost, ctx->stream));
     // a coarse table has a bucket for every priority, so push_k reports none as fresh: the batch's priorities are
@@ -1132,7 +1200,8 @@ int push_impl(hqs_ctx* ctx, u32 n, const u32* task, u32 first_handle, const u32*
     std::vector<u64> fresh;
     if (ctx->coarse) distinct_priorities(priority, n, fresh);
     CU(cudaStreamSynchronize(ctx->stream));
-    if (ctx->h_small[1]) return fail(ctx, HQS_E_INVALID, "a class id of the batch is >= n_classes %u (nothing was pushed)", ctx->Q);
+    if (ctx->h_small[1] & 1u) return fail(ctx, HQS_E_INVALID, "a class id of the batch is >= n_classes %u (nothing was pushed)", ctx->Q);
+    if (ctx->h_small[1]) return fail(ctx, HQS_E_INVALID, "a handle of the batch is a live task (nothing was pushed)");
     ctx->n_handles = std::max(ctx->n_handles, max_h + 1);
     ctx->stats.n_handles = ctx->n_handles;
     const u32 newcnt = ctx->h_small[0];
@@ -1237,17 +1306,14 @@ int hqs_ready_remove(hqs_ctx* ctx, uint32_t n, const uint32_t* task) {
     if (n == 0) return HQS_OK;
     if (!task) return fail(ctx, HQS_E_INVALID, "null task array");
     CU(cudaSetDevice(ctx->device));
-    if (n > ctx->push_cap) {
-        CU(cudaStreamSynchronize(ctx->stream));
-        if (ctx->d_push_task) { CU(cudaFree(ctx->d_push_task)); CU(cudaFree(ctx->d_push_cls)); CU(cudaFree(ctx->d_push_prio)); }
-        ctx->push_cap = std::max<u32>(n, 1u << 16);
-        CU(cudaMalloc(&ctx->d_push_task, (size_t)ctx->push_cap * 4));
-        CU(cudaMalloc(&ctx->d_push_cls, (size_t)ctx->push_cap * 4));
-        CU(cudaMalloc(&ctx->d_push_prio, (size_t)ctx->push_cap * 8));
-    }
+    if (int rc_ = ensure_push_staging(ctx, n)) return rc_;
     CU(cudaMemcpyAsync(ctx->d_push_task, task, (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream));
     remove_k<<<(n + 255) / 256, 256, 0, ctx->stream>>>(n, ctx->d_push_task, ctx->d_key, ctx->n_handles);
     ctx->stats.kernel_launches++;
+    if (ctx->graph_storage) {   // the removed tasks' consumer lists go (their consumers wait until the host cancels them)
+        graph_unlink_k<<<(n + 255) / 256, 256, 0, ctx->stream>>>(n, ctx->d_push_task, ctx->n_handles, ctx->d_ghead);
+        ctx->stats.kernel_launches++;
+    }
     CU(cudaGetLastError());
     CU(cudaStreamSynchronize(ctx->stream));
     return HQS_OK;
@@ -1296,6 +1362,7 @@ int hqs_dag_load(hqs_ctx* ctx, uint32_t n_tasks, const uint32_t* class_id, const
     if (!ctx) return HQS_E_INVALID;
     if (!n_tasks || !class_id || !priority || !n_deps || !cons_off) return fail(ctx, HQS_E_INVALID, "null DAG arrays");
     if (ctx->Q == 0) return fail(ctx, HQS_E_STATE, "hqs_classes_set has not been called");
+    if (ctx->graph) return fail(ctx, HQS_E_STATE, "hqs_dag_load is not available after hqs_graph_push");
     const u32 n_edges = cons_off[n_tasks];
     if (n_edges && !cons) return fail(ctx, HQS_E_INVALID, "null consumer array");
     for (u32 i = 0; i < n_tasks; ++i)
@@ -1342,15 +1409,10 @@ int hqs_tasks_finished(hqs_ctx* ctx, uint32_t n, const uint32_t* task, uint32_t*
     if (!ctx->dag) return fail(ctx, HQS_E_STATE, "hqs_tasks_finished needs hqs_dag_load");
     if (n == 0) return HQS_OK;
     if (!task) return fail(ctx, HQS_E_INVALID, "null task array");
+    for (u32 i = 0; i < n; ++i)
+        if (task[i] >= ctx->n_handles) return fail(ctx, HQS_E_INVALID, "task %u >= n_tasks %u (nothing was finished)", task[i], ctx->n_handles);
     CU(cudaSetDevice(ctx->device));
-    if (n > ctx->push_cap) {
-        CU(cudaStreamSynchronize(ctx->stream));
-        if (ctx->d_push_task) { CU(cudaFree(ctx->d_push_task)); CU(cudaFree(ctx->d_push_cls)); CU(cudaFree(ctx->d_push_prio)); }
-        ctx->push_cap = std::max<u32>(n, 1u << 16);
-        CU(cudaMalloc(&ctx->d_push_task, (size_t)ctx->push_cap * 4));
-        CU(cudaMalloc(&ctx->d_push_cls, (size_t)ctx->push_cap * 4));
-        CU(cudaMalloc(&ctx->d_push_prio, (size_t)ctx->push_cap * 8));
-    }
+    if (int rc_ = ensure_push_staging(ctx, n)) return rc_;
     CU(cudaMemcpyAsync(ctx->d_push_task, task, (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream));
     CU(cudaMemsetAsync(ctx->d_newcnt, 0, sizeof(u32), ctx->stream));
     finished_k<<<(n + 255) / 256, 256, 0, ctx->stream>>>(n, ctx->d_push_task, ctx->d_cons_off, ctx->d_cons, ctx->d_deps,
@@ -1362,6 +1424,234 @@ int hqs_tasks_finished(hqs_ctx* ctx, uint32_t n, const uint32_t* task, uint32_t*
         CU(cudaStreamSynchronize(ctx->stream));
         *n_new_ready = ctx->h_small[0];
     }
+    return HQS_OK;
+}
+
+}  // extern "C"
+
+namespace {
+// the context states in which the graph calls are refused
+int graph_mode_check(hqs_ctx* ctx, const char* what) {
+    if (ctx->dag) return fail(ctx, HQS_E_STATE, "%s is not available after hqs_dag_load", what);
+    if (ctx->x_world) return fail(ctx, HQS_E_STATE, "%s is not available on a sharded ready set", what);
+    if (ctx->tick_pending) return fail(ctx, HQS_E_STATE, "the previous tick has not been fetched");
+    return HQS_OK;
+}
+
+// Before a push whose edges do not fit: the pool keeps only the edges whose consumer still waits on their incarnation,
+// rewritten list by list into a fresh pool of max(capacity, 2 * live + n_edges) slots.
+int graph_compact(hqs_ctx* ctx, u32 n_edges) {
+    const u32 nb = (ctx->n_handles + GRAPH_PER_BLOCK - 1) / GRAPH_PER_BLOCK;
+    u32 live = 0;
+    if (nb) {
+        graph_gc_count_k<<<nb, GRAPH_NT, 0, ctx->stream>>>(ctx->n_handles, ctx->d_ghead, ctx->d_pool, ctx->d_key, ctx->d_ggen, ctx->d_gblk);
+        graph_scan_k<<<1, 1024, 0, ctx->stream>>>(nb, ctx->d_gblk, ctx->d_gsmall + 2);
+        ctx->stats.kernel_launches += 2;
+        CU(cudaGetLastError());
+        CU(cudaMemcpyAsync(ctx->h_small + 4, ctx->d_gsmall + 2, sizeof(u32), cudaMemcpyDeviceToHost, ctx->stream));
+        CU(cudaStreamSynchronize(ctx->stream));
+        live = ctx->h_small[4];
+    }
+    const u64 want = std::max<u64>(ctx->pool_cap, 2ull * live + n_edges);
+    if (want >= GRAPH_NIL) return fail(ctx, HQS_E_LIMIT, "the edge pool would need %llu slots", (unsigned long long)want);
+    GraphEdge* fresh = nullptr;
+    CU(cudaMalloc(&fresh, (size_t)want * sizeof(GraphEdge)));
+    if (nb) {
+        graph_gc_move_k<<<nb, GRAPH_NT, 0, ctx->stream>>>(ctx->n_handles, ctx->d_ghead, ctx->d_pool, fresh, ctx->d_key, ctx->d_ggen, ctx->d_gblk);
+        ctx->stats.kernel_launches++;
+        CU(cudaGetLastError());
+    }
+    CU(cudaStreamSynchronize(ctx->stream));
+    CU(cudaFree(ctx->d_pool));
+    ctx->d_pool = fresh;
+    ctx->pool_cap = (u32)want;
+    ctx->pool_used = live;
+    ctx->pool_compactions++;
+    return HQS_OK;
+}
+
+// the device half of hqs_graph_push's validation on its own, before a compaction (a rejected batch changes nothing)
+int graph_prevalidate(hqs_ctx* ctx, u32 n, const u32* task, const u32* class_id) {
+    if (int rc = ensure_push_staging(ctx, n)) return rc;
+    CU(cudaMemcpyAsync(ctx->d_push_task, task, (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream));
+    CU(cudaMemcpyAsync(ctx->d_push_cls, class_id, (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream));
+    CU(cudaMemsetAsync(ctx->d_newcnt, 0, 2 * sizeof(u32), ctx->stream));
+    push_validate_k<<<(n + 255) / 256, 256, 0, ctx->stream>>>(n, ctx->d_push_cls, ctx->Q, ctx->d_newcnt);
+    graph_validate_k<<<(n + 255) / 256, 256, 0, ctx->stream>>>(n, ctx->d_push_task, ctx->d_key, ctx->n_handles, ctx->d_newcnt);
+    ctx->stats.kernel_launches += 2;
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(ctx->h_small, ctx->d_newcnt, 2 * sizeof(u32), cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+    if (ctx->h_small[1] & 1u) return fail(ctx, HQS_E_INVALID, "a class id of the batch is >= n_classes %u (nothing was pushed)", ctx->Q);
+    if (ctx->h_small[1]) return fail(ctx, HQS_E_INVALID, "a handle of the batch is a live task (nothing was pushed)");
+    return HQS_OK;
+}
+
+// duplicates among the k dependencies d[0..k)
+bool has_duplicate(const u32* d, u32 k, std::vector<u32>& scratch) {
+    if (k <= 16) {
+        for (u32 a = 1; a < k; ++a)
+            for (u32 b = 0; b < a; ++b)
+                if (d[a] == d[b]) return true;
+        return false;
+    }
+    scratch.assign(d, d + k);
+    std::sort(scratch.begin(), scratch.end());
+    return std::adjacent_find(scratch.begin(), scratch.end()) != scratch.end();
+}
+}  // namespace
+
+extern "C" {
+
+int hqs_graph_push(hqs_ctx* ctx, uint32_t n, const uint32_t* task, const uint32_t* class_id, const uint64_t* priority,
+                   const uint32_t* dep_off, const uint32_t* deps, uint32_t* n_ready) {
+    if (!ctx) return HQS_E_INVALID;
+    if (n_ready) *n_ready = 0;
+    if (int rc = graph_mode_check(ctx, "hqs_graph_push")) return rc;
+    if (n == 0) return HQS_OK;
+    if (!task || !class_id || !priority || !dep_off) return fail(ctx, HQS_E_INVALID, "null task arrays");
+    if (ctx->Q == 0) return fail(ctx, HQS_E_STATE, "hqs_classes_set has not been called");
+    // host-knowable checks, then the batch's own dependency lists: the handle -> batch position map is a range test when
+    // the handles are consecutive (a job's tasks), a sorted table otherwise
+    if (dep_off[0] != 0) return fail(ctx, HQS_E_INVALID, "dep_off[0] = %u, not 0", dep_off[0]);
+    for (u32 i = 0; i < n; ++i)
+        if (dep_off[i + 1] < dep_off[i]) return fail(ctx, HQS_E_INVALID, "dep_off decreases at task %u", i);
+    const u32 m = dep_off[n];
+    if (m && !deps) return fail(ctx, HQS_E_INVALID, "null dependency array");
+    bool range = true;
+    for (u32 i = 0; i < n; ++i) {
+        if (task[i] == GRAPH_NIL) return fail(ctx, HQS_E_INVALID, "task handle 0xFFFFFFFF is reserved");
+        range &= task[i] == task[0] + i;
+    }
+    std::vector<std::pair<u32, u32>>& pos = ctx->g_pos;
+    if (!range) {
+        pos.resize(n);
+        for (u32 i = 0; i < n; ++i) pos[i] = {task[i], i};
+        std::sort(pos.begin(), pos.end());
+        for (u32 i = 1; i < n; ++i)
+            if (pos[i].first == pos[i - 1].first) return fail(ctx, HQS_E_INVALID, "handle %u appears twice in the batch", pos[i].first);
+    }
+    auto batch_pos = [&](u32 h) -> u32 {      // position of h in the batch, GRAPH_NIL if it is not in it
+        if (range) return h - task[0] < n ? h - task[0] : GRAPH_NIL;
+        auto it = std::lower_bound(pos.begin(), pos.end(), std::make_pair(h, 0u));
+        return it != pos.end() && it->first == h ? it->second : GRAPH_NIL;
+    };
+    std::vector<u32>& off = ctx->g_off;
+    std::vector<u32>& dep = ctx->g_dep;
+    std::vector<u32> scratch;
+    off.resize((size_t)n + 1);
+    dep.clear();
+    dep.reserve(m);
+    off[0] = 0;
+    for (u32 i = 0; i < n; ++i) {
+        const u32 lo = dep_off[i], hi = dep_off[i + 1];
+        if (has_duplicate(deps + lo, hi - lo, scratch)) return fail(ctx, HQS_E_INVALID, "task %u names a dependency twice", task[i]);
+        for (u32 j = lo; j < hi; ++j) {
+            const u32 d = deps[j];
+            if (d == task[i]) return fail(ctx, HQS_E_INVALID, "task %u depends on itself", d);
+            const u32 p = batch_pos(d);
+            if (p == GRAPH_NIL) {
+                if (d >= ctx->n_handles) return fail(ctx, HQS_E_INVALID, "dependency %u of task %u is unknown", d, task[i]);
+                dep.push_back(d);                // counts if VALID on the device
+            } else if (p < i) {
+                dep.push_back(d);                // an earlier task of the batch
+            }                                    // a later one is dropped, as on_new_tasks does
+        }
+        off[i + 1] = (u32)dep.size();
+    }
+    const u32 me = (u32)dep.size();
+    CU(cudaSetDevice(ctx->device));
+    int rc;
+    if ((rc = ensure_graph_storage(ctx))) return rc;
+    // a push that allocates or compacts the pool is validated on the device first, so that a rejected batch changes nothing
+    if (!ctx->d_pool || (u64)ctx->pool_used + me > ctx->pool_cap)
+        if ((rc = graph_prevalidate(ctx, n, task, class_id))) return rc;
+    if (!ctx->d_pool) {
+        const u64 cap = std::max<u64>(2ull * me, GRAPH_POOL_MIN);
+        if (cap >= GRAPH_NIL) return fail(ctx, HQS_E_LIMIT, "the edge pool would need %llu slots", (unsigned long long)cap);
+        CU(cudaMalloc(&ctx->d_pool, (size_t)cap * sizeof(GraphEdge)));
+        ctx->pool_cap = (u32)cap;
+        ctx->pool_used = 0;
+    } else if ((u64)ctx->pool_used + me > ctx->pool_cap) {
+        if ((rc = graph_compact(ctx, me))) return rc;
+    }
+    const size_t stage = (size_t)n + 1 + me;
+    if (stage > ctx->gstage_cap) {
+        const size_t cap = std::max<size_t>(stage * 2, 1u << 16);
+        if ((rc = dev_realloc(ctx, &ctx->d_gstage, 0, cap, false, false))) return rc;
+        ctx->gstage_cap = cap;
+    }
+    // pageable sources: staged by the runtime before the calls return
+    CU(cudaMemcpyAsync(ctx->d_gstage, off.data(), ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, ctx->stream));
+    if (me) CU(cudaMemcpyAsync(ctx->d_gstage + n + 1, dep.data(), (size_t)me * 4, cudaMemcpyHostToDevice, ctx->stream));
+    const GraphBatch g{ctx->pool_used};
+    if ((rc = push_impl(ctx, n, task, 0, class_id, priority, &g))) return rc;
+    ctx->pool_used += me;
+    ctx->graph = true;
+    if (n_ready) *n_ready = ctx->h_small[2];
+    return HQS_OK;
+}
+
+int hqs_graph_finished(hqs_ctx* ctx, uint32_t n, const uint32_t* task, const uint32_t** new_ready, uint32_t* n_new_ready) {
+    if (!ctx) return HQS_E_INVALID;
+    ctx->g_new_ready.clear();
+    if (new_ready) *new_ready = ctx->g_new_ready.data();
+    if (n_new_ready) *n_new_ready = 0;
+    if (int rc = graph_mode_check(ctx, "hqs_graph_finished")) return rc;
+    if (n == 0) return HQS_OK;
+    if (!task) return fail(ctx, HQS_E_INVALID, "null task array");
+    for (u32 i = 0; i < n; ++i)
+        if (task[i] >= ctx->n_handles) return fail(ctx, HQS_E_INVALID, "task %u >= n_handles %u (nothing was finished)", task[i], ctx->n_handles);
+    CU(cudaSetDevice(ctx->device));
+    int rc;
+    if ((rc = ensure_graph_storage(ctx))) return rc;
+    if ((rc = ensure_push_staging(ctx, n))) return rc;
+    u32* win = ctx->d_push_cls;          // the staging of class ids is free during this call
+    CU(cudaMemcpyAsync(ctx->d_push_task, task, (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream));
+    graph_leave_k<<<(n + 255) / 256, 256, 0, ctx->stream>>>(n, ctx->d_push_task, ctx->d_key, win);
+    graph_release_k<<<(n + 255) / 256, 256, 0, ctx->stream>>>(n, win, ctx->d_key, ctx->d_gdeps, ctx->d_ggen, ctx->d_ghead,
+                                                              ctx->d_pool, ctx->d_gbits);
+    const u32 n_words = (ctx->n_handles + 31) / 32, nb = (n_words + GRAPH_PER_BLOCK - 1) / GRAPH_PER_BLOCK;
+    graph_ready_count_k<<<nb, GRAPH_NT, 0, ctx->stream>>>(n_words, ctx->d_gbits, ctx->d_gblk);
+    graph_scan_k<<<1, 1024, 0, ctx->stream>>>(nb, ctx->d_gblk, ctx->d_gsmall + 1);
+    graph_ready_emit_k<<<nb, GRAPH_NT, 0, ctx->stream>>>(n_words, ctx->d_gbits, ctx->d_gblk, ctx->d_gready);
+    ctx->stats.kernel_launches += 5;
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(ctx->h_small + 3, ctx->d_gsmall + 1, sizeof(u32), cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+    const u32 k = ctx->h_small[3];
+    ctx->g_new_ready.resize(k);
+    if (k) {
+        CU(cudaMemcpyAsync(ctx->g_new_ready.data(), ctx->d_gready, (size_t)k * 4, cudaMemcpyDeviceToHost, ctx->stream));
+        CU(cudaStreamSynchronize(ctx->stream));
+    }
+    if (new_ready) *new_ready = ctx->g_new_ready.data();
+    if (n_new_ready) *n_new_ready = k;
+    return HQS_OK;
+}
+
+int hqs_graph_debug(hqs_ctx* ctx, uint64_t out[4]) {
+    if (!ctx || !out) return HQS_E_INVALID;
+    if (int rc = graph_mode_check(ctx, "hqs_graph_debug")) return rc;
+    CU(cudaSetDevice(ctx->device));
+    unsigned long long* d_out = nullptr;
+    CU(cudaMalloc(&d_out, 2 * sizeof(unsigned long long)));
+    unsigned long long h[2] = {0, 0};
+    cudaError_t e = cudaMemsetAsync(d_out, 0, sizeof h, ctx->stream);
+    if (e == cudaSuccess && ctx->n_handles) {
+        graph_debug_k<<<(ctx->n_handles + 255) / 256, 256, 0, ctx->stream>>>(ctx->n_handles, ctx->d_key,
+                                                                           ctx->graph_storage ? ctx->d_ghead : nullptr, ctx->d_pool, d_out);
+        ctx->stats.kernel_launches++;
+        e = cudaGetLastError();
+    }
+    if (e == cudaSuccess) e = cudaMemcpyAsync(h, d_out, sizeof h, cudaMemcpyDeviceToHost, ctx->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+    cudaFree(d_out);
+    if (e != cudaSuccess) return fail(ctx, HQS_E_CUDA, "hqs_graph_debug: %s", cudaGetErrorString(e));
+    out[0] = h[0];
+    out[1] = ctx->pool_cap;
+    out[2] = ctx->pool_compactions;
+    out[3] = h[1];
     return HQS_OK;
 }
 

@@ -117,6 +117,12 @@ void GpuCore::on_new_tasks(std::vector<TaskId> tasks) {
     for (const TaskId& t : tasks) handle_of(t);
 }
 
+size_t GpuCore::n_waiting() const {
+    size_t n = 0;
+    for (const TaskState& t : tasks_) n += t.waiting ? 1 : 0;
+    return n;
+}
+
 // A task that was never announced through on_new_tasks gets its handle on first use (arrival order).
 uint32_t GpuCore::handle_of(TaskId task) {
     auto it = handle_of_.find(task.as_u64());
@@ -141,16 +147,27 @@ void GpuCore::remove_ready_task(TaskId task) {
     if (it == handle_of_.end()) return;
     const uint32_t h = it->second;
     tasks_[h].live = false;
+    tasks_[h].waiting = false;
     // still in the host-side batch?
     for (size_t i = 0; i < push_h_.size(); ++i)
         if (push_h_[i] == h) {
             push_h_.erase(push_h_.begin() + i); push_c_.erase(push_c_.begin() + i); push_p_.erase(push_p_.begin() + i);
             return;
         }
+    for (size_t i = 0; i < graph_h_.size(); ++i)
+        if (graph_h_[i] == h) {
+            graph_h_.erase(graph_h_.begin() + i); graph_c_.erase(graph_c_.begin() + i); graph_p_.erase(graph_p_.begin() + i);
+            graph_deps_.erase(graph_deps_.begin() + i);
+            return;
+        }
     if (hqs_ready_remove(ctx_, 1, &h) != HQS_OK) { last_error_ = hqs_last_error(ctx_); log_error("hqs_ready_remove", last_error_.c_str()); }
 }
 
 void GpuCore::flush_ready() {
+    if (graph_flush_) {                     // the core has submitted tasks with dependencies (tako_shim_graph.cpp)
+        (this->*graph_flush_)();
+        return;
+    }
     if (!forget_h_.empty()) {
         // finished tasks leave the device table for good, so their handles stop pinning priority levels (the device
         // prunes levels without tasks: tako priorities carry a per-job component)

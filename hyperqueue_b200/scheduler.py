@@ -15,6 +15,8 @@ parity tests and the benchmark read like the reference's own tests:
   WorkerTaskMapping::send_messages  mapping.rs:255-288      GpuScheduler.run_scheduling_grouped -> GroupedTaskMapping
   Worker::insert_sn_task         worker.rs:188-196          (free vectors come back from the device)
   task_finished / remove_sn_task reactor.rs:500-580         GpuScheduler.tasks_finished
+  on_new_tasks with dependencies reactor.rs:188-220         GpuScheduler.submit_tasks
+  task_finished in a task graph  reactor.rs:500-580         GpuScheduler.graph_tasks_finished
 
 Device memory, streams and the kernels live in libhqsched_b200.so; this module only marshals numpy
 arrays.  No CPU fallback exists: without the library or a CUDA device every call raises.
@@ -558,6 +560,52 @@ class GpuScheduler:
             self._check(self._lib.hqs_tasks_finished(self._ctx, h.size, L.ptr(h), C.byref(n_new)))
             return int(n_new.value)
         return 0
+
+    def submit_tasks(self, handles, rq_ids, priorities, dep_off, deps) -> int:
+        """on_new_tasks (reactor.rs:188-220) for new tasks with dependencies (hqs_graph_push): the dependencies of
+        handles[i] are deps[dep_off[i]:dep_off[i + 1]].  A dependency on a live task or on an earlier task of the batch
+        counts; one on a finished, removed or unknown task, or on a later task of the batch, is dropped.  Returns how many of
+        the tasks are ready at once; the others wait until graph_tasks_finished releases them."""
+        h = np.ascontiguousarray(handles, dtype=np.uint32)
+        c = np.ascontiguousarray(rq_ids, dtype=np.uint32)
+        p = np.ascontiguousarray(priorities, dtype=np.uint64)
+        off = np.ascontiguousarray(dep_off, dtype=np.uint32)
+        d = np.ascontiguousarray(deps, dtype=np.uint32)
+        if not (h.shape == c.shape == p.shape) or off.shape != (h.size + 1,):
+            raise ValueError("shape mismatch")
+        if h.size == 0:
+            return 0
+        self._sync_classes()
+        n_ready = C.c_uint32(0)
+        self._check(self._lib.hqs_graph_push(self._ctx, h.size, L.ptr(h), L.ptr(c), L.ptr(p), L.ptr(off),
+                                             L.ptr(d) if d.size else None, C.byref(n_ready)))
+        self._grow_tasks(int(h.max()) + 1)
+        self._task_class[h] = c
+        self._task_prio[h] = p
+        return int(n_ready.value)
+
+    def graph_tasks_finished(self, handles) -> np.ndarray:
+        """task_finished for tasks of a task graph (hqs_graph_finished): returns each assigned task's resources to its
+        worker, as tasks_finished does, takes the tasks out of the ready set and releases their consumers.  Returns the
+        handles that became ready, ascending."""
+        h = np.ascontiguousarray(handles, dtype=np.uint32)
+        if h.size == 0:
+            return np.zeros(0, dtype=np.uint32)
+        ptr = C.POINTER(C.c_uint32)()
+        k = C.c_uint32(0)
+        self._check(self._lib.hqs_graph_finished(self._ctx, h.size, L.ptr(h), C.byref(ptr), C.byref(k)))
+        ready = np.ctypeslib.as_array(ptr, shape=(k.value,)).copy() if k.value else np.zeros(0, dtype=np.uint32)
+        self._grow_tasks(int(h.max()) + 1)
+        assigned = h[self._task_worker[h] >= 0]
+        if assigned.size:
+            return_resources(self, np.unique(assigned))
+        return ready
+
+    def graph_debug(self) -> np.ndarray:
+        """hqs_graph_debug: [live edges, edge-pool capacity, pool compactions, waiting tasks]."""
+        out = (C.c_uint64 * 4)()
+        self._check(self._lib.hqs_graph_debug(self._ctx, out))
+        return np.array(list(out), dtype=np.uint64)
 
     def new_worker_query(self, worker_totals: np.ndarray, now: float = 0.0, remaining_s: Optional[np.ndarray] = None,
                          min_utilization: Optional[np.ndarray] = None):

@@ -179,8 +179,39 @@ int hqs_ready_remove(hqs_ctx* ctx, uint32_t n, const uint32_t* task);
 int hqs_dag_load(hqs_ctx* ctx, uint32_t n_tasks, const uint32_t* class_id, const uint64_t* priority,
                  const uint32_t* n_deps, const uint32_t* cons_off, const uint32_t* cons);
 /* task_finished for n tasks: decrements unfinished_deps of every consumer; consumers reaching zero
- * become ready (add_ready_task).  *n_new_ready (optional) receives how many did. */
+ * become ready (add_ready_task).  *n_new_ready (optional) receives how many did.  A handle >= n_tasks rejects the batch
+ * (HQS_E_INVALID, nothing changed). */
 int hqs_tasks_finished(hqs_ctx* ctx, uint32_t n, const uint32_t* task, uint32_t* n_new_ready);
+
+/* Task graphs that grow while the ready set runs (reactor.rs:188-220 on_new_tasks, :500-580 task_finished): jobs with
+ * dependencies are submitted between ticks into the same table that hqs_ready_push fills.
+ * hqs_graph_push: on_new_tasks for n NEW tasks with dependencies.  task[i], class_id[i], priority[i] as in hqs_ready_push
+ * (priorities are registered the same way); the dependencies of task i are deps[dep_off[i] .. dep_off[i+1]) (handles).
+ * A dependency counts if its handle is VALID (waiting, ready, or assigned and not finished) or is an EARLIER task of the
+ * batch; one on a later task of the batch, or on a handle that finished, was removed or never pushed, is dropped, as
+ * on_new_tasks drops a dependency it does not find.  A task without a counted dependency is READY at once, the others wait
+ * (VALID, neither READY nor DONE).  *n_ready (optional) = how many of the n tasks are ready at once.
+ * HQS_E_INVALID with nothing changed: a class id >= n_classes; a handle 0xFFFFFFFF, a handle twice in the batch, or a
+ * handle that is VALID; a task that depends on itself or names a dependency twice; a dependency that is neither in the
+ * batch nor < n_handles; dep_off not starting at 0 or decreasing.
+ * hqs_graph_finished: task_finished for n tasks: each leaves the table (like hqs_ready_remove), and then each consumer still
+ * waiting on the incarnation it was submitted with loses a dependency; the ones reaching zero become READY.  *new_ready
+ * points to their handles, ASCENDING, in a buffer the context owns, valid until the next call on the context;
+ * *n_new_ready is their number.  A handle >= n_handles rejects the batch (HQS_E_INVALID, nothing changed); a handle that
+ * is not VALID is ignored (tako's "unknown task finished"); a handle named twice counts once.  A consumer finished in the
+ * same batch is not released.
+ * Handle re-use: a task that leaves the table (hqs_graph_finished or hqs_ready_remove) takes its consumer list with it.
+ * The consumers of a REMOVED task keep waiting until the host removes them too (tako cancels the consumers of a cancelled
+ * task).  A handle that is submitted again is a new incarnation: the producers of the old one never release it.
+ * hqs_ready_push / _range / _remove / _rearm, prefill, ticks, queries and the grouped fetch work unchanged on a graph
+ * context.  HQS_E_STATE: the graph calls after hqs_dag_load, on a context attached with hqs_shard_attach, or while a tick or
+ * query is pending; hqs_dag_load after a graph push.
+ * hqs_graph_debug (debug / test aid, like hqs_debug_keys): out[0] live edges (linked into a producer's consumer list),
+ * out[1] edge-pool capacity, out[2] pool compactions so far, out[3] waiting tasks (VALID, not READY, not DONE). */
+int hqs_graph_push(hqs_ctx* ctx, uint32_t n, const uint32_t* task, const uint32_t* class_id, const uint64_t* priority,
+                   const uint32_t* dep_off, const uint32_t* deps, uint32_t* n_ready);
+int hqs_graph_finished(hqs_ctx* ctx, uint32_t n, const uint32_t* task, const uint32_t** new_ready, uint32_t* n_new_ready);
+int hqs_graph_debug(hqs_ctx* ctx, uint64_t out[4]);
 
 /* One scheduler tick over the current ready set (replaces run_scheduling_solver + the task-selection
  * half of create_task_mapping).

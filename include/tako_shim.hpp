@@ -12,6 +12,7 @@
 //   on_new_worker / on_remove_worker (reactor.rs:20-32, 64-186)       GpuCore::on_new_worker / on_remove_worker
 //   Worker::block_request / unblock (worker.rs:328-344)               GpuCore::block_request / unblock_request
 //   on_new_tasks (reactor.rs:188-220)                                 GpuCore::on_new_tasks (handles in TaskId order)
+//   on_new_tasks with dependencies (reactor.rs:188-220)               GpuCore::on_new_tasks(std::vector<NewTask>)
 //   TaskQueues::add_ready_task (taskqueue.rs:37-43)                   GpuCore::add_ready_task
 //   TaskQueue::remove (taskqueue.rs:194-216)                          GpuCore::remove_ready_task
 //   run_scheduling_inner (main.rs:40-46) -> WorkerTaskMapping         GpuCore::run_scheduling
@@ -71,6 +72,13 @@ struct ResourceRequestVariants {          // request.rs:229-353
     std::vector<ResourceRequest> variants;
 };
 
+struct NewTask {                          // a submitted task with its dependencies (task.rs:22-43, reactor.rs:188-220)
+    TaskId id;
+    ResourceRqId rq = 0;
+    Priority priority = 0;
+    std::vector<TaskId> deps;
+};
+
 struct WorkerTaskUpdate {                 // mapping.rs:9-14
     std::vector<std::pair<TaskId, ResourceVariantId>> assigned;   // priority descending (mapping.rs:125-128)
     std::vector<TaskId> prefills;         // ComputeTasks entries with variant = None, sent BEFORE the assigned ones (mapping.rs:264-275)
@@ -106,6 +114,13 @@ public:
 
     // on_new_tasks (reactor.rs:188-220): announces the tasks of a submit; handles are assigned in ascending TaskId
     void on_new_tasks(std::vector<TaskId> tasks);
+    // on_new_tasks for tasks with dependencies: handles are assigned in TaskId order; a dependency on an unknown, finished
+    // or cancelled task is dropped (reactor.rs:197-204), one on a live task (waiting, ready, assigned or running) counts.
+    // Tasks without a counted dependency become ready; the others wait until their producers finish.  The tasks go to the
+    // device in one hqs_graph_push at the next flush, and from then on this core's finished tasks release their consumers
+    // through hqs_graph_finished.
+    void on_new_tasks(std::vector<NewTask> tasks);
+    size_t n_waiting() const;             // tasks waiting for a dependency
     void add_ready_task(TaskId task, ResourceRqId rq, Priority priority);
     void remove_ready_task(TaskId task);
 
@@ -145,7 +160,8 @@ private:
         Priority priority = 0;
         int64_t worker = -1;              // TaskRuntimeState::Assigned{worker_id, rv_id} (task.rs:22-43)
         ResourceVariantId variant = 0;
-        bool live = false;
+        bool live = false;                // in the ready set, assigned or running
+        bool waiting = false;             // submitted with a dependency that has not finished yet
         int64_t prefilled_on = -1;        // TaskRuntimeState::Prefilled{worker_id}
         int64_t retracting_from = -1;     // TaskRuntimeState::Retracting{worker_id}
     };
@@ -159,6 +175,7 @@ private:
     void apply_free_after(const TickInput& in);
     void flush_classes();
     void flush_ready();
+    void flush_graph();
     uint32_t handle_of(TaskId task);
 
     hqs_ctx* ctx_ = nullptr;
@@ -172,6 +189,13 @@ private:
     std::vector<uint32_t> push_h_, push_c_;
     std::vector<uint32_t> forget_h_;                         // finished tasks: leave the device table at the next flush
     std::vector<uint64_t> push_p_;
+    // graph submits batched until the next flush: handle, class, priority, dependency handles
+    std::vector<uint32_t> graph_h_, graph_c_;
+    std::vector<uint64_t> graph_p_;
+    std::vector<std::vector<uint32_t>> graph_deps_;
+    // set by the first submit with dependencies: the flush pushes the graph batch and sends finishes through
+    // hqs_graph_finished (both in tako_shim_graph.cpp)
+    void (GpuCore::*graph_flush_)() = nullptr;
     std::vector<hqs_assignment> out_;
     uint32_t pf_max_ = 0;
     std::map<uint64_t, std::pair<WorkerId, ResourceVariantId>> redirects_;
@@ -188,6 +212,11 @@ int hqshim_selftest(int device, int verbose);
 // one grouped, through a multi-class drain with priorities and through proactive filling with retract / redirect; every
 // tick's mappings must be equal, list order included, and so must the free vectors.  Returns the number of failed checks.
 int hqshim_selftest_grouped(int device, int verbose);
+// Self-test of GpuCore's task graphs on CUDA device `device` (tako_shim_graph.cpp): seeded random jobs with dependencies on
+// earlier jobs, submitted between ticks of a zero-duration drain, with cancellations; every task runs once, never before a
+// dependency that was live at its submit finished, and the host mirror's waiting set matches the device's.  Returns the
+// number of failed checks.
+int hqshim_selftest_graph(int device, int verbose);
 // Measuring aid (tools/grouped_probe.py): host wall time of one tick INCLUDING the construction of the per-worker lists of a
 // WorkerTaskMapping, on a context the caller has loaded (handles stand in for TaskIds).  grouped = 0: hqs_tick and one map
 // lookup + push_back per record of the flat stream; grouped = 1: hqs_tick_grouped and one lookup + reserved append per worker,
