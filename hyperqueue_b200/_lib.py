@@ -29,7 +29,7 @@ ABI_SYMBOLS = [
     "hqs_query_fetch", "hqs_shard_query_launch", "hqs_shard_query_solve",
     "hqs_tick_fetch_grouped", "hqs_tick_grouped", "hqs_grouped_reserve", "hqs_grouped_kernel_ms",
     "hqs_levels_live", "hqs_levels_retain",
-    "hqs_graph_push", "hqs_graph_finished", "hqs_graph_debug",
+    "hqs_graph_push", "hqs_graph_finished", "hqs_graph_cancel", "hqs_graph_debug",
 ]
 HQS_IPC_HANDLE_BYTES = 64
 
@@ -97,6 +97,8 @@ def load_shim() -> C.CDLL:
         _shim.hqshim_selftest_grouped.restype = C.c_int
         _shim.hqshim_selftest_graph.argtypes = [C.c_int, C.c_int]
         _shim.hqshim_selftest_graph.restype = C.c_int
+        _shim.hqshim_selftest_graph_cancel.argtypes = [C.c_int, C.c_int]
+        _shim.hqshim_selftest_graph_cancel.restype = C.c_int
         _shim.hqshim_time_mapping.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_int,
                                               C.c_uint32, C.c_void_p, C.POINTER(C.c_uint64)]
         _shim.hqshim_time_mapping.restype = C.c_int
@@ -127,6 +129,7 @@ def load_library() -> C.CDLL:
     lib.hqs_tasks_finished.argtypes = [vp, u32, u32p, C.POINTER(C.c_uint32)]
     lib.hqs_graph_push.argtypes = [vp, u32, u32p, u32p, u64p, u32p, u32p, C.POINTER(C.c_uint32)]
     lib.hqs_graph_finished.argtypes = [vp, u32, u32p, C.POINTER(C.POINTER(C.c_uint32)), C.POINTER(C.c_uint32)]
+    lib.hqs_graph_cancel.argtypes = [vp, u32, u32p, C.POINTER(C.POINTER(C.c_uint32)), C.POINTER(C.c_uint32)]
     lib.hqs_graph_debug.argtypes = [vp, C.POINTER(C.c_uint64)]
     lib.hqs_tick.argtypes = [vp, u32, vp, u64p, u64p, u8p, u32, vp, C.POINTER(C.c_uint32), u64p]
     lib.hqs_tick_launch.argtypes = [vp, u32, vp, u64p, u64p, u8p, u32]

@@ -1,6 +1,6 @@
 // hqs_graph.cuh — task graphs that grow while the ready set runs: hqs_graph_push / hqs_graph_finished (on_new_tasks and
-// task_finished, reactor.rs:188-220, 500-580).  Included by hqsched.cu inside its anonymous namespace, after
-// hqs_ready_set.cuh.
+// task_finished, reactor.rs:188-220, 500-580) and hqs_graph_cancel (on_cancel_tasks / task_failed, reactor.rs:596-770).
+// Included by hqsched.cu inside its anonymous namespace, after hqs_ready_set.cuh and hqs_solver.cuh.
 //
 // Per handle h (allocated at the first graph push, grown with the task table):
 //   gdeps[h]  u32  unfinished counted dependencies of h's current incarnation
@@ -8,7 +8,8 @@
 //   ghead[h]  u32  first edge of h's consumer list, GRAPH_NIL = none
 // Edge pool: GraphEdge {consumer, consumer's incarnation, next}.  A push takes its slots by the batch's dependency offsets
 // (no atomics) and links each counted edge in front of its producer's list.  A list is emptied whenever its producer
-// leaves the table (finished or removed), so head[h] != GRAPH_NIL implies that h is VALID.
+// leaves the table (finished, removed or cancelled), so head[h] != GRAPH_NIL implies that h is VALID.
+// hqs_graph_cancel also keeps gwork[h] (a work list of n_handles slots, GRAPH_NIL between calls).
 #pragma once
 
 constexpr u32 GRAPH_NIL = ~0u;
@@ -250,5 +251,154 @@ __global__ void graph_debug_k(u32 n_handles, const u32* __restrict__ key, const 
     if ((threadIdx.x & 31) == 0) {
         if (edges) atomicAdd(&out[0], (unsigned long long)edges);
         if (waiting) atomicAdd(&out[1], (unsigned long long)waiting);
+    }
+}
+
+// hqs_graph_cancel: the named VALID handles and, transitively, every consumer still waiting on its edge's incarnation are
+// marked in the bitmap `bits` and appended to the work list `work` (a handle is admitted by winning its bit, so the list
+// never holds a handle twice and never wraps).  The marking kernel's counters sit on separate lines: idle warps poll them.
+struct GraphCancelSync {
+    u32 tail, pad0[31];      // entries appended to the work list
+    u32 head, pad1[31];      // entries taken from it
+    u32 pending, pad2[31];   // entries admitted and not yet walked (queued or in a warp)
+    u32 steps, pad3[31];     // entries walked so far: the progress the idle warps' time-outs watch
+    u32 done, error, pad4[30];   // done: the marking drained the list; error: the wait that timed out (1 the list, 2 a slot)
+};
+constexpr u32 GRAPH_CANCEL_NT = 256;
+
+// the named handles that are VALID seed the work list (host-checked: every handle < n_handles)
+__global__ void graph_cancel_seed_k(u32 n, const u32* __restrict__ task, const u32* __restrict__ key, u32* __restrict__ bits,
+                                    u32* __restrict__ work, GraphCancelSync* __restrict__ s) {
+    const u32 i = blockIdx.x * blockDim.x + threadIdx.x, lane = threadIdx.x & 31;
+    u32 h = GRAPH_NIL;
+    bool won = false;
+    if (i < n) {
+        h = task[i];
+        const u32 b = 1u << (h & 31);
+        won = (key[h] & KEY_VALID) && !(atomicOr(&bits[h >> 5], b) & b);      // a handle named twice is admitted once
+    }
+    const u32 m = __ballot_sync(0xffffffffu, won);
+    if (!m) return;
+    const u32 lead = __ffs(m) - 1;
+    u32 base = 0;
+    if (lane == lead) {
+        atomicAdd(&s->pending, __popc(m));
+        base = atomicAdd(&s->tail, __popc(m));
+    }
+    base = __shfl_sync(0xffffffffu, base, lead);
+    if (won) work[base + __popc(m & ((1u << lane) - 1))] = h;
+}
+
+// lane 0: the next entry of the work list, GRAPH_NIL once the list is drained (nothing queued, no warp walking) or a wait
+// timed out.  The time-outs count time without progress (no entry appended or walked), so a long chain never trips them.
+__device__ u32 graph_cancel_pop(const u32* work, GraphCancelSync* s) {
+    long long t0 = clock64();
+    u32 seen_tail = ld_acquire(&s->tail), seen_steps = ld_acquire(&s->steps);
+    for (;;) {
+        if (ld_acquire(&s->error)) return GRAPH_NIL;
+        const u32 hd = ld_acquire(&s->head), tl = ld_acquire(&s->tail);
+        if (hd < tl) {
+            if (atomicCAS(&s->head, hd, hd + 1) != hd) continue;
+            const long long t1 = clock64();      // the slot is reserved; its appender writes it next
+            u32 v;
+            while ((v = ld_acquire(&work[hd])) == GRAPH_NIL)
+                if (clock64() - t1 > SPIN_TIMEOUT_CYCLES) { atomicCAS(&s->error, 0u, 2u); return GRAPH_NIL; }
+            return v;
+        }
+        if (ld_acquire(&s->pending) == 0) {   // zero is final: only a warp holding an entry admits new ones
+            s->done = 1u;
+            return GRAPH_NIL;
+        }
+        const u32 st = ld_acquire(&s->steps);
+        if (st != seen_steps || tl != seen_tail) {
+            seen_steps = st;
+            seen_tail = tl;
+            t0 = clock64();
+        } else if (clock64() - t0 > SPIN_TIMEOUT_CYCLES) {
+            atomicCAS(&s->error, 0u, 1u);
+            return GRAPH_NIL;
+        }
+        __nanosleep(100);
+    }
+}
+
+// The marking: one cooperative launch, every warp a worker.  A warp walks its entry's consumer list (lane 0 follows the
+// links, 32 edges at a time, and every lane tests one edge), admits each consumer that still waits on the edge's incarnation
+// and wins its bit, keeps the first one it admits to walk next (a chain never goes through the list) and appends the rest.
+// So the work list holds only part of the closure; the bitmap holds all of it.
+// key, ggen, ghead and pool are only read: nothing leaves the table before graph_cancel_apply_k.
+__global__ void __launch_bounds__(GRAPH_CANCEL_NT) graph_cancel_mark_k(const u32* __restrict__ key, const u32* __restrict__ ggen,
+                                                                        const u32* __restrict__ ghead,
+                                                                        const GraphEdge* __restrict__ pool, u32* bits, u32* work,
+                                                                        GraphCancelSync* s) {
+    __shared__ u32 s_cons[GRAPH_CANCEL_NT], s_gen[GRAPH_CANCEL_NT];
+    const u32 lane = threadIdx.x & 31, w0 = threadIdx.x & ~31u;
+    u32 h = GRAPH_NIL;                                  // warp-uniform: the entry being walked
+    for (;;) {
+        if (h == GRAPH_NIL) {
+            if (lane == 0) h = graph_cancel_pop(work, s);
+            h = __shfl_sync(0xffffffffu, h, 0);
+            if (h == GRAPH_NIL) return;
+        }
+        u32 e = ghead[h], next = GRAPH_NIL;
+        while (e != GRAPH_NIL) {
+            u32 cnt = 0;
+            if (lane == 0)
+                for (; cnt < 32 && e != GRAPH_NIL; ++cnt) {
+                    const GraphEdge E = pool[e];
+                    s_cons[w0 + cnt] = E.cons;
+                    s_gen[w0 + cnt] = E.gen;
+                    e = E.next;
+                }
+            e = __shfl_sync(0xffffffffu, e, 0);
+            cnt = __shfl_sync(0xffffffffu, cnt, 0);
+            __syncwarp();
+            bool won = false;
+            u32 c = 0;
+            if (lane < cnt) {
+                c = s_cons[w0 + lane];
+                const u32 b = 1u << (c & 31);
+                won = ggen[c] == s_gen[w0 + lane] && (key[c] & (KEY_VALID | KEY_READY | KEY_DONE)) == KEY_VALID &&
+                      !(atomicOr(&bits[c >> 5], b) & b);
+            }
+            __syncwarp();
+            u32 m = __ballot_sync(0xffffffffu, won);
+            if (m && next == GRAPH_NIL) {               // the first admitted consumer inherits this entry's pending count
+                const u32 first = __ffs(m) - 1;
+                next = __shfl_sync(0xffffffffu, c, first);
+                m &= m - 1;
+                won = won && lane != first;
+            }
+            if (m) {                                    // counted as pending before anyone can take them
+                const u32 lead = __ffs(m) - 1;
+                u32 base = 0;
+                if (lane == lead) {
+                    atomicAdd(&s->pending, __popc(m));
+                    base = atomicAdd(&s->tail, __popc(m));
+                }
+                base = __shfl_sync(0xffffffffu, base, lead);
+                if (won) st_release(&work[base + __popc(m & ((1u << lane) - 1))], c);
+            }
+        }
+        if (lane == 0) {
+            atomicAdd(&s->steps, 1u);
+            if (next == GRAPH_NIL) atomicSub(&s->pending, 1u);
+        }
+        h = next;
+    }
+}
+
+// After the ordered emit (graph_ready_emit_k wrote the marked handles ascending to out[0 .. *n_out) and cleared the bitmap),
+// and only if the marking drained its list: every marked handle leaves the table (as graph_leave_k makes it leave) and its
+// consumer list is emptied.  The work list returns to GRAPH_NIL either way.
+__global__ void graph_cancel_apply_k(u32* __restrict__ work, const GraphCancelSync* __restrict__ s, const u32* __restrict__ out,
+                                     const u32* __restrict__ n_out, u32* __restrict__ key, u32* __restrict__ ghead) {
+    const u32 stride = gridDim.x * blockDim.x, i0 = blockIdx.x * blockDim.x + threadIdx.x;
+    for (u32 i = i0, n = s->tail; i < n; i += stride) work[i] = GRAPH_NIL;
+    if (!s->done || s->error) return;
+    for (u32 i = i0, n = *n_out; i < n; i += stride) {
+        const u32 h = out[i];
+        key[h] &= ~(KEY_READY | KEY_VALID | KEY_DONE | KEY_PF);
+        ghead[h] = GRAPH_NIL;
     }
 }

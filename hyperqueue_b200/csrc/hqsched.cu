@@ -15,7 +15,8 @@
 //   key[h]   u32  bit31 READY | bit30 DONE (assigned by a tick) | bit29 VALID | bit28 PREFILLED | level(14) | class(14)
 //   prio[h]  u64  tako Priority (only read when the level table changes)
 //   deps[h]  u32  unfinished dependencies (DAG mode), cons_off/cons: CSR of consumers
-//   gdeps[h], ggen[h], ghead[h] + an edge pool: task graphs grown by hqs_graph_push (hqs_graph.cuh)
+//   gdeps[h], ggen[h], ghead[h] + an edge pool: task graphs grown by hqs_graph_push (hqs_graph.cuh); gwork[h]: the work
+//            list of hqs_graph_cancel
 // One tick = ONE cooperative kernel (tick_k, hqs_tick.cuh):
 //   worker CTAs : per-chunk histogram of ready tasks by group g = level*Q + class (HBM streaming, 4 B/task), exclusive
 //                 scan of the chunk table over chunks, on request the pack step (one warp fills one worker), then the
@@ -53,8 +54,8 @@ typedef uint32_t u32;
 typedef uint64_t u64;
 
 #include "hqs_ready_set.cuh"
-#include "hqs_graph.cuh"
 #include "hqs_solver.cuh"
+#include "hqs_graph.cuh"
 #include "hqs_tick.cuh"
 #include "hqs_group.cuh"
 
@@ -127,7 +128,9 @@ struct hqs_ctx {
     u32* d_gstage = nullptr; size_t gstage_cap = 0;   // a push's dependency offsets [n + 1] and dependencies
     std::vector<u32> g_off, g_dep;      // host scratch of hqs_graph_push
     std::vector<std::pair<u32, u32>> g_pos;
-    std::vector<u32> g_new_ready;       // what *new_ready of hqs_graph_finished points to
+    std::vector<u32> g_new_ready;       // what *new_ready of hqs_graph_finished / *cancelled of hqs_graph_cancel points to
+    u32* d_gwork = nullptr;             // [cap_handles] work list of hqs_graph_cancel's marking (GRAPH_NIL between calls)
+    GraphCancelSync* d_gcsync = nullptr;
     // push staging (device)
     u32* d_push_task = nullptr; u32* d_push_cls = nullptr; u64* d_push_prio = nullptr;
     u32 push_cap = 0;
@@ -232,6 +235,8 @@ int ensure_handles(hqs_ctx* ctx, u32 need) {
         if ((rc = dev_realloc(ctx, &ctx->d_gbits, ctx->cap_handles / 32, cap / 32, true, true))) return rc;
         if ((rc = dev_realloc(ctx, &ctx->d_gready, 0, cap, false, false))) return rc;
         if ((rc = dev_realloc(ctx, &ctx->d_gblk, 0, cap / GRAPH_PER_BLOCK + 1, false, false))) return rc;
+        if ((rc = dev_realloc(ctx, &ctx->d_gwork, 0, cap, false, false))) return rc;
+        CU(cudaMemsetAsync(ctx->d_gwork, 0xFF, (size_t)cap * 4, ctx->stream));
     }
     ctx->cap_handles = cap;
     return HQS_OK;
@@ -243,6 +248,7 @@ int ensure_graph_storage(hqs_ctx* ctx) {
     const u32 cap = ctx->cap_handles;
     int rc;
     if (!ctx->d_gsmall) CU(cudaMalloc(&ctx->d_gsmall, 4 * sizeof(u32)));
+    if (!ctx->d_gcsync) CU(cudaMalloc(&ctx->d_gcsync, sizeof(GraphCancelSync)));
     if ((rc = dev_realloc(ctx, &ctx->d_gdeps, 0, cap, false, true))) return rc;
     if ((rc = dev_realloc(ctx, &ctx->d_ggen, 0, cap, false, true))) return rc;
     if ((rc = dev_realloc(ctx, &ctx->d_ghead, 0, cap, false, false))) return rc;
@@ -250,6 +256,8 @@ int ensure_graph_storage(hqs_ctx* ctx) {
     if ((rc = dev_realloc(ctx, &ctx->d_gbits, 0, cap / 32, false, true))) return rc;
     if ((rc = dev_realloc(ctx, &ctx->d_gready, 0, cap, false, false))) return rc;
     if ((rc = dev_realloc(ctx, &ctx->d_gblk, 0, cap / GRAPH_PER_BLOCK + 1, false, false))) return rc;
+    if ((rc = dev_realloc(ctx, &ctx->d_gwork, 0, cap, false, false))) return rc;
+    CU(cudaMemsetAsync(ctx->d_gwork, 0xFF, (size_t)cap * 4, ctx->stream));
     ctx->graph_storage = true;
     return HQS_OK;
 }
@@ -1033,7 +1041,7 @@ void hqs_destroy(hqs_ctx* ctx) {
                         ctx->d_seg_wv, ctx->d_out, ctx->d_hdr, ctx->d_free_after, ctx->d_tickin, ctx->d_sync, ctx->d_pk_fr,
                         ctx->d_pk_quota, ctx->d_pk_taken, ctx->d_pk_cand, ctx->d_pk_meta, ctx->d_prune_lv, ctx->d_prune_live,
                         ctx->d_gdeps, ctx->d_ggen, ctx->d_ghead, ctx->d_gbits, ctx->d_gready, ctx->d_gblk, ctx->d_gsmall,
-                        ctx->d_pool, ctx->d_gstage};
+                        ctx->d_pool, ctx->d_gstage, ctx->d_gwork, ctx->d_gcsync};
     for (void* p : dev_ptrs) if (p) cudaFree(p);
     for (void* p : ctx->x_opened) cudaIpcCloseMemHandle(p);
     if (ctx->d_xbuf) cudaFree(ctx->d_xbuf);
@@ -1627,6 +1635,59 @@ int hqs_graph_finished(hqs_ctx* ctx, uint32_t n, const uint32_t* task, const uin
     }
     if (new_ready) *new_ready = ctx->g_new_ready.data();
     if (n_new_ready) *n_new_ready = k;
+    return HQS_OK;
+}
+
+int hqs_graph_cancel(hqs_ctx* ctx, uint32_t n, const uint32_t* task, const uint32_t** cancelled, uint32_t* n_cancelled) {
+    if (!ctx) return HQS_E_INVALID;
+    ctx->g_new_ready.clear();
+    if (cancelled) *cancelled = ctx->g_new_ready.data();
+    if (n_cancelled) *n_cancelled = 0;
+    if (int rc = graph_mode_check(ctx, "hqs_graph_cancel")) return rc;
+    if (n == 0) return HQS_OK;
+    if (!task) return fail(ctx, HQS_E_INVALID, "null task array");
+    for (u32 i = 0; i < n; ++i)
+        if (task[i] >= ctx->n_handles) return fail(ctx, HQS_E_INVALID, "task %u >= n_handles %u (nothing was cancelled)", task[i], ctx->n_handles);
+    CU(cudaSetDevice(ctx->device));
+    int rc;
+    if ((rc = ensure_graph_storage(ctx))) return rc;
+    if ((rc = ensure_push_staging(ctx, n))) return rc;
+    CU(cudaMemcpyAsync(ctx->d_push_task, task, (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream));
+    CU(cudaMemsetAsync(ctx->d_gcsync, 0, sizeof(GraphCancelSync), ctx->stream));
+    // the launches do not depend on the depth of the closure: seed, marking (the whole closure), ordered emit, apply
+    graph_cancel_seed_k<<<(n + 255) / 256, 256, 0, ctx->stream>>>(n, ctx->d_push_task, ctx->d_key, ctx->d_gbits, ctx->d_gwork,
+                                                                  ctx->d_gcsync);
+    {
+        const u32* key = ctx->d_key; const u32* ggen = ctx->d_ggen; const u32* ghead = ctx->d_ghead;
+        const GraphEdge* pool = ctx->d_pool;
+        u32* bits = ctx->d_gbits; u32* work = ctx->d_gwork; GraphCancelSync* sync = ctx->d_gcsync;
+        void* kargs[] = {&key, &ggen, &ghead, &pool, &bits, &work, &sync};
+        CU(cudaLaunchCooperativeKernel((const void*)graph_cancel_mark_k, dim3(ctx->grid_ctas), dim3(GRAPH_CANCEL_NT), kargs, 0,
+                                       ctx->stream));
+    }
+    const u32 n_words = (ctx->n_handles + 31) / 32, nb = (n_words + GRAPH_PER_BLOCK - 1) / GRAPH_PER_BLOCK;
+    graph_ready_count_k<<<nb, GRAPH_NT, 0, ctx->stream>>>(n_words, ctx->d_gbits, ctx->d_gblk);
+    graph_scan_k<<<1, 1024, 0, ctx->stream>>>(nb, ctx->d_gblk, ctx->d_gsmall + 1);
+    graph_ready_emit_k<<<nb, GRAPH_NT, 0, ctx->stream>>>(n_words, ctx->d_gbits, ctx->d_gblk, ctx->d_gready);
+    graph_cancel_apply_k<<<ctx->sm_count * 4, 256, 0, ctx->stream>>>(ctx->d_gwork, ctx->d_gcsync, ctx->d_gready, ctx->d_gsmall + 1,
+                                                                     ctx->d_key, ctx->d_ghead);
+    ctx->stats.kernel_launches += 6;
+    CU(cudaGetLastError());
+    GraphCancelSync hs;
+    CU(cudaMemcpyAsync(&hs, ctx->d_gcsync, sizeof hs, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaMemcpyAsync(ctx->h_small + 3, ctx->d_gsmall + 1, sizeof(u32), cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+    if (hs.error || !hs.done)
+        return fail(ctx, HQS_E_CUDA, "a wait of the cancel marking kernel timed out (%s; %u handles marked, nothing was cancelled)",
+                    hs.error == 2 ? "a work-list slot that was never written" : "the work list made no progress", hs.tail);
+    const u32 k = ctx->h_small[3];
+    ctx->g_new_ready.resize(k);
+    if (k) {
+        CU(cudaMemcpyAsync(ctx->g_new_ready.data(), ctx->d_gready, (size_t)k * 4, cudaMemcpyDeviceToHost, ctx->stream));
+        CU(cudaStreamSynchronize(ctx->stream));
+    }
+    if (cancelled) *cancelled = ctx->g_new_ready.data();
+    if (n_cancelled) *n_cancelled = k;
     return HQS_OK;
 }
 

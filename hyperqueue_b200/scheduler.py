@@ -17,6 +17,7 @@ parity tests and the benchmark read like the reference's own tests:
   task_finished / remove_sn_task reactor.rs:500-580         GpuScheduler.tasks_finished
   on_new_tasks with dependencies reactor.rs:188-220         GpuScheduler.submit_tasks
   task_finished in a task graph  reactor.rs:500-580         GpuScheduler.graph_tasks_finished
+  on_cancel_tasks / task_failed  reactor.rs:596-770         GpuScheduler.graph_cancel_tasks
 
 Device memory, streams and the kernels live in libhqsched_b200.so; this module only marshals numpy
 arrays.  No CPU fallback exists: without the library or a CUDA device every call raises.
@@ -600,6 +601,42 @@ class GpuScheduler:
         if assigned.size:
             return_resources(self, np.unique(assigned))
         return ready
+
+    def graph_cancel_tasks(self, handles) -> Tuple[np.ndarray, Dict[int, List[int]]]:
+        """on_cancel_tasks (reactor.rs:696-770) over a task graph (hqs_graph_cancel): the named tasks that are live and,
+        transitively, every consumer still waiting on them leave the ready set.  For a named task that is assigned, its
+        resources go back to its worker; prefilled, it is no longer held; retracting, its redirect is dropped and the
+        resources taken on the redirect target come back.  Returns (every handle that left, ascending; worker id -> the
+        named tasks to cancel there, in the order they were named: the CancelTasks messages).  The consumers are the
+        returned handles that were not named; they were waiting, so no worker holds them.  A failed task (task_failed,
+        reactor.rs:596-694) is cancelled the same way; its worker gets no message."""
+        h = np.ascontiguousarray(handles, dtype=np.uint32)
+        if h.size == 0:
+            return np.zeros(0, dtype=np.uint32), {}
+        ptr = C.POINTER(C.c_uint32)()
+        k = C.c_uint32(0)
+        self._check(self._lib.hqs_graph_cancel(self._ctx, h.size, L.ptr(h), C.byref(ptr), C.byref(k)))
+        gone = np.ctypeslib.as_array(ptr, shape=(k.value,)).copy() if k.value else np.zeros(0, dtype=np.uint32)
+        self._grow_tasks(int(h.max()) + 1)
+        left = set(gone.tolist())
+        messages: Dict[int, List[int]] = {}
+        assigned = []
+        for t in dict.fromkeys(h.tolist()):
+            if t not in left:
+                continue                                     # "Task is not here"
+            if t in self._retracting_from:
+                messages.setdefault(self._retracting_from.pop(t), []).append(t)
+                self.redirects.pop(t, None)
+                assigned.append(t)                           # try_remove_redirection: the target's resources come back
+            elif self._task_worker[t] >= 0:
+                messages.setdefault(int(self.worker_ids[self._task_worker[t]]), []).append(t)
+                assigned.append(t)
+            elif self._pf_worker[t] >= 0:
+                messages.setdefault(int(self._pf_worker[t]), []).append(t)
+                self._pf_worker[t] = -1
+        if assigned:
+            return_resources(self, np.array(assigned, dtype=np.int64))
+        return gone, messages
 
     def graph_debug(self) -> np.ndarray:
         """hqs_graph_debug: [live edges, edge-pool capacity, pool compactions, waiting tasks]."""

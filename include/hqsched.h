@@ -200,9 +200,21 @@ int hqs_tasks_finished(hqs_ctx* ctx, uint32_t n, const uint32_t* task, uint32_t*
  * *n_new_ready is their number.  A handle >= n_handles rejects the batch (HQS_E_INVALID, nothing changed); a handle that
  * is not VALID is ignored (tako's "unknown task finished"); a handle named twice counts once.  A consumer finished in the
  * same batch is not released.
- * Handle re-use: a task that leaves the table (hqs_graph_finished or hqs_ready_remove) takes its consumer list with it.
- * The consumers of a REMOVED task keep waiting until the host removes them too (tako cancels the consumers of a cancelled
- * task).  A handle that is submitted again is a new incarnation: the producers of the old one never release it.
+ * Handle re-use: a task that leaves the table (hqs_graph_finished, hqs_ready_remove or hqs_graph_cancel) takes its consumer
+ * list with it.  The consumers of a task removed with hqs_ready_remove keep waiting until the host removes them too;
+ * hqs_graph_cancel removes a task together with its consumers.  A handle that is submitted again is a new incarnation: the
+ * producers of the old one never release it.
+ * hqs_graph_cancel: on_cancel_tasks / task_failed (reactor.rs:596-770) for n tasks.  Every named handle that is VALID
+ * (waiting, ready, prefilled or assigned) leaves the table, and so does, transitively, every consumer still waiting on the
+ * incarnation its edge was made for (a consumer cancelled or resubmitted since is not followed).  Leaving is what
+ * hqs_graph_finished does to a task (READY, VALID, DONE and PREFILLED cleared, so it stops pinning its priority level)
+ * without releasing anyone; the consumer lists of all of them are emptied.  *cancelled points to every handle that left,
+ * ASCENDING (the named VALID ones and the consumers reached), in the buffer hqs_graph_finished uses, valid until the next
+ * call on the context; *n_cancelled is their number.  The consumers are that list without the named handles.  A handle
+ * that is not VALID is ignored, a handle named twice counts once.  HQS_E_INVALID with nothing changed: a handle >=
+ * n_handles, or task == NULL with n > 0.  The number of kernel launches does not depend on the depth of the graph (one
+ * cooperative kernel marks the whole closure); a marking that makes no progress for about a second fails with
+ * HQS_E_CUDA and changes nothing.
  * hqs_ready_push / _range / _remove / _rearm, prefill, ticks, queries and the grouped fetch work unchanged on a graph
  * context.  HQS_E_STATE: the graph calls after hqs_dag_load, on a context attached with hqs_shard_attach, or while a tick or
  * query is pending; hqs_dag_load after a graph push.
@@ -211,6 +223,7 @@ int hqs_tasks_finished(hqs_ctx* ctx, uint32_t n, const uint32_t* task, uint32_t*
 int hqs_graph_push(hqs_ctx* ctx, uint32_t n, const uint32_t* task, const uint32_t* class_id, const uint64_t* priority,
                    const uint32_t* dep_off, const uint32_t* deps, uint32_t* n_ready);
 int hqs_graph_finished(hqs_ctx* ctx, uint32_t n, const uint32_t* task, const uint32_t** new_ready, uint32_t* n_new_ready);
+int hqs_graph_cancel(hqs_ctx* ctx, uint32_t n, const uint32_t* task, const uint32_t** cancelled, uint32_t* n_cancelled);
 int hqs_graph_debug(hqs_ctx* ctx, uint64_t out[4]);
 
 /* One scheduler tick over the current ready set (replaces run_scheduling_solver + the task-selection

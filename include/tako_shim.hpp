@@ -19,6 +19,8 @@
 //   WorkerTaskMapping / WorkerTaskUpdate (mapping.rs:9-21)            same names
 //   task_finished -> Worker::remove_sn_task (reactor.rs:500-580,      GpuCore::on_task_finished
 //                    workerload.rs:194-202)
+//   on_cancel_tasks (reactor.rs:696-770)                              GpuCore::on_cancel_tasks
+//   task_failed (reactor.rs:596-694)                                  GpuCore::on_task_failed
 //
 // Error behaviour follows the reference: the scheduler never returns errors to its caller.  A failing tick logs
 // the library's message and schedules nothing (solver.rs:412-415); invalid requests ("Zero resources cannot be
@@ -84,6 +86,10 @@ struct WorkerTaskUpdate {                 // mapping.rs:9-14
     std::vector<TaskId> prefills;         // ComputeTasks entries with variant = None, sent BEFORE the assigned ones (mapping.rs:264-275)
     std::vector<TaskId> retracts;         // one RetractTasks message, sent first (mapping.rs:257-262)
 };
+struct CancelledTasks {                   // on_cancel_tasks (reactor.rs:696-770)
+    std::vector<TaskId> cancelled;        // every task that left, the named ones and their consumers, ascending TaskId
+    std::map<WorkerId, std::vector<TaskId>> messages;   // CancelTasks per worker, tasks in the order they were named
+};
 struct WorkerTaskMapping {                // mapping.rs:16-21
     std::map<WorkerId, WorkerTaskUpdate> workers;
     size_t n_assigned() const {
@@ -130,6 +136,15 @@ public:
     // push_back per record.  Defined in tako_shim_grouped.cpp.
     WorkerTaskMapping run_scheduling_grouped(uint64_t now_ms = 0);
     void on_task_finished(TaskId task);
+    // on_cancel_tasks (reactor.rs:696-770): the named tasks that are known and not finished leave, and so do, transitively,
+    // all their waiting consumers (hqs_graph_cancel; a core that never submitted dependencies has none).  An assigned or
+    // running task gives its resources back and is cancelled on its worker, a prefilled one on the worker holding it, a
+    // retracting one on the worker it is being retracted from (its redirect is dropped and the target's resources come
+    // back).  Pending submits and finishes are flushed first.  Defined in tako_shim_graph_cancel.cpp.
+    CancelledTasks on_cancel_tasks(const std::vector<TaskId>& tasks);
+    // task_failed (reactor.rs:596-694): the failing task leaves as a cancelled one does, without a message to its worker;
+    // returns its transitive consumers, ascending TaskId (the list tako hands to on_task_error), which left with it.
+    std::vector<TaskId> on_task_failed(TaskId task);
 
     // SchedulerConfig::proactive_filling_reserve / _max (scheduler/state.rs:14-21).  tako's defaults are 16 / 40; this
     // class starts with proactive filling OFF (max = 0) and the embedding server switches it on.
@@ -177,6 +192,8 @@ private:
     void flush_ready();
     void flush_graph();
     uint32_t handle_of(TaskId task);
+    std::vector<uint32_t> cancel_on_device(const std::vector<uint32_t>& handles);
+    int64_t leave_worker(TaskState& t);
 
     hqs_ctx* ctx_ = nullptr;
     uint32_t R_;
@@ -217,6 +234,11 @@ int hqshim_selftest_grouped(int device, int verbose);
 // dependency that was live at its submit finished, and the host mirror's waiting set matches the device's.  Returns the
 // number of failed checks.
 int hqshim_selftest_graph(int device, int verbose);
+// Self-test of GpuCore::on_cancel_tasks / on_task_failed on CUDA device `device` (tako_shim_graph_cancel.cpp): seeded random
+// jobs with dependencies in a zero-duration drain with proactive filling on, random cancels of tasks in every state and
+// failures of assigned tasks.  Every task runs once or is reported as left exactly once, the reported consumers equal the
+// test's own closure, and the free vectors return to the totals.  Returns the number of failed checks.
+int hqshim_selftest_graph_cancel(int device, int verbose);
 // Measuring aid (tools/grouped_probe.py): host wall time of one tick INCLUDING the construction of the per-worker lists of a
 // WorkerTaskMapping, on a context the caller has loaded (handles stand in for TaskIds).  grouped = 0: hqs_tick and one map
 // lookup + push_back per record of the flat stream; grouped = 1: hqs_tick_grouped and one lookup + reserved append per worker,
