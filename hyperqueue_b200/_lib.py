@@ -30,6 +30,8 @@ ABI_SYMBOLS = [
     "hqs_tick_fetch_grouped", "hqs_tick_grouped", "hqs_grouped_reserve", "hqs_grouped_kernel_ms",
     "hqs_levels_live", "hqs_levels_retain",
     "hqs_graph_push", "hqs_graph_finished", "hqs_graph_cancel", "hqs_graph_debug",
+    "hqs_shard_graph_init", "hqs_shard_graph_push", "hqs_shard_graph_finished", "hqs_shard_graph_cancel",
+    "hqs_shard_graph_remove",
 ]
 HQS_IPC_HANDLE_BYTES = 64
 
@@ -131,6 +133,11 @@ def load_library() -> C.CDLL:
     lib.hqs_graph_finished.argtypes = [vp, u32, u32p, C.POINTER(C.POINTER(C.c_uint32)), C.POINTER(C.c_uint32)]
     lib.hqs_graph_cancel.argtypes = [vp, u32, u32p, C.POINTER(C.POINTER(C.c_uint32)), C.POINTER(C.c_uint32)]
     lib.hqs_graph_debug.argtypes = [vp, C.POINTER(C.c_uint64)]
+    lib.hqs_shard_graph_init.argtypes = [vp, u32, u32, u32]
+    lib.hqs_shard_graph_push.argtypes = [vp, u32, u32p, u32p, u64p, u32p, u32p, C.POINTER(C.c_uint32)]
+    lib.hqs_shard_graph_finished.argtypes = [vp, u32, u32p, C.POINTER(C.POINTER(C.c_uint32)), C.POINTER(C.c_uint32)]
+    lib.hqs_shard_graph_cancel.argtypes = [vp, u32, u32p, C.POINTER(C.POINTER(C.c_uint32)), C.POINTER(C.c_uint32)]
+    lib.hqs_shard_graph_remove.argtypes = [vp, u32, u32p]
     lib.hqs_tick.argtypes = [vp, u32, vp, u64p, u64p, u8p, u32, vp, C.POINTER(C.c_uint32), u64p]
     lib.hqs_tick_launch.argtypes = [vp, u32, vp, u64p, u64p, u8p, u32]
     lib.hqs_tick_fetch.argtypes = [vp, u32, vp, C.POINTER(C.c_uint32), u64p]

@@ -10,6 +10,12 @@
 // (no atomics) and links each counted edge in front of its producer's list.  A list is emptied whenever its producer
 // leaves the table (finished, removed or cancelled), so head[h] != GRAPH_NIL implies that h is VALID.
 // hqs_graph_cancel also keeps gwork[h] (a work list of n_handles slots, GRAPH_NIL between calls).
+//
+// A sharded graph context (hqs_shard_graph_init) keeps all of the above replicated, indexed by the GLOBAL handle
+// (0 .. n_total), plus gvalid[h], one bit per handle: h is VALID in the graph's view.  Its key table holds only the handles
+// it owns, [lo, hi), at key[h - lo].  Every rank makes every graph call with the same arguments and runs the same kernels on
+// the same replicated state, so the replicas stay equal; each rank writes only the keys it owns and reports only the
+// handles it owns.  The kernels take both forms through GraphKeys and a template flag S (false: one context).
 #pragma once
 
 constexpr u32 GRAPH_NIL = ~0u;
@@ -23,6 +29,43 @@ struct GraphEdge {
     u32 gen;    // the consumer's incarnation the edge was made for
     u32 next;   // next edge of the producer's list
 };
+
+// Where the graph kernels read VALID and write keys.  S = false (one context): key[h] for every handle.  S = true (a sharded
+// graph context): VALID is the replicated bit gvalid[h], a VALID task waits while it has unfinished dependencies (nothing
+// but a release makes a task with dependencies READY there: hqs_ready_push is refused), and only the handles
+// [lo, hi) have a key, key[h - lo] (hi is clipped to the key table's capacity: the keys beyond it are not VALID).
+struct GraphKeys {
+    u32* key;
+    u32* gvalid;     // S only: [n_total / 32] bits
+    u32 lo, hi;
+};
+
+template <bool S>
+__device__ __forceinline__ bool graph_valid(const GraphKeys& k, u32 h) {
+    if (S) return (k.gvalid[h >> 5] >> (h & 31)) & 1u;
+    return k.key[h] & KEY_VALID;
+}
+
+// h is VALID and neither READY nor DONE
+template <bool S>
+__device__ __forceinline__ bool graph_waiting(const GraphKeys& k, const u32* gdeps, u32 h) {
+    if (S) return graph_valid<true>(k, h) && gdeps[h] != 0u;
+    return (k.key[h] & (KEY_VALID | KEY_READY | KEY_DONE)) == KEY_VALID;
+}
+
+// the key word of h if this context holds it, nullptr otherwise
+template <bool S>
+__device__ __forceinline__ u32* graph_own(const GraphKeys& k, u32 h) {
+    if (!S) return k.key + h;
+    return h - k.lo < k.hi - k.lo ? k.key + (h - k.lo) : nullptr;
+}
+
+// host: runs f(std::true_type) for a sharded graph context, f(std::false_type) otherwise (the kernel instance to launch)
+template <typename F>
+void graph_dispatch(bool shard, F&& f) {
+    if (shard) f(std::true_type{});
+    else f(std::false_type{});
+}
 
 // exclusive prefix sum over the block (NT <= 1024); *total receives the block's sum in every thread
 template <u32 NT>
@@ -70,20 +113,29 @@ __global__ void __launch_bounds__(1024) graph_scan_k(u32 nb, u32* __restrict__ b
 
 // a pushed handle that is still VALID rejects the batch (flag[1] bit 1; push_k and graph_link_k then write nothing).
 // Handles >= n_handles have never been pushed.
-__global__ void graph_validate_k(u32 n, const u32* __restrict__ task, const u32* __restrict__ key, u32 n_handles,
+template <bool S>
+__global__ void graph_validate_k(u32 n, const u32* __restrict__ task, const GraphKeys k, u32 n_handles,
                                  u32* __restrict__ flag) {
     const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
     const u32 h = i < n ? task[i] : GRAPH_NIL;
-    const bool bad = h < n_handles && (key[h] & KEY_VALID);
+    const bool bad = h < n_handles && graph_valid<S>(k, h);
     if (__ballot_sync(0xffffffffu, bad) && (threadIdx.x & 31) == 0) atomicOr(&flag[1], 2u);
+}
+
+// sharded graph context, after graph_validate_k: the batch becomes VALID in the graph's view (push_k's part for the replica)
+__global__ void graph_enter_k(u32 n, const u32* __restrict__ task, const u32* __restrict__ flag, u32* __restrict__ gvalid) {
+    if (flag[1]) return;                    // the batch was rejected
+    const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) atomicOr(&gvalid[task[i] >> 5], 1u << (task[i] & 31));
 }
 
 // after push_k: task i's dependencies are dep[off[i] .. off[i+1]) (the host dropped those on later tasks of the batch).  One
 // counts if its producer is VALID: a task of the table or an earlier task of the batch (push_k made those VALID).  Counted
 // edges take slot e0 + j and are linked into the producer's list; a task with a counted dependency is waiting (READY
-// cleared).  n_ready[0] += tasks ready at once.
+// cleared).  n_ready[0] += tasks ready at once (of this context's own handles).
+template <bool S>
 __global__ void graph_link_k(u32 n, const u32* __restrict__ task, const u32* __restrict__ off, const u32* __restrict__ dep,
-                             u32 e0, const u32* __restrict__ flag, u32* key, u32* __restrict__ gdeps,
+                             u32 e0, const u32* __restrict__ flag, const GraphKeys k, u32* __restrict__ gdeps,
                              u32* __restrict__ ggen, u32* __restrict__ ghead, GraphEdge* __restrict__ pool,
                              u32* __restrict__ n_ready) {
     if (flag[1]) return;                    // the batch was rejected
@@ -96,7 +148,7 @@ __global__ void graph_link_k(u32 n, const u32* __restrict__ task, const u32* __r
         u32 cnt = 0;
         for (u32 j = off[i], hi = off[i + 1]; j < hi; ++j) {
             const u32 p = dep[j];
-            if (!(key[p] & KEY_VALID)) continue;            // finished, removed or never pushed: dropped
+            if (!graph_valid<S>(k, p)) continue;            // finished, removed or never pushed: dropped
             const u32 e = e0 + j;
             pool[e].cons = h;
             pool[e].gen = g;
@@ -104,8 +156,9 @@ __global__ void graph_link_k(u32 n, const u32* __restrict__ task, const u32* __r
             ++cnt;
         }
         gdeps[h] = cnt;
-        if (cnt) key[h] &= ~KEY_READY;      // only this thread writes key[h]; the others read its VALID bit
-        ready = cnt == 0;
+        u32* kh = graph_own<S>(k, h);
+        if (cnt && kh) *kh &= ~KEY_READY;   // only this thread writes key[h]; the others read its VALID bit
+        ready = cnt == 0 && kh;
     }
     const u32 made = __popc(__ballot_sync(0xffffffffu, ready));
     if ((threadIdx.x & 31) == 0 && made) atomicAdd(n_ready, made);
@@ -114,22 +167,34 @@ __global__ void graph_link_k(u32 n, const u32* __restrict__ task, const u32* __r
 // hqs_graph_finished, phase 1: every finished task leaves the table.  Only the thread that clears VALID keeps the handle
 // (win[i]), so a handle named twice, or one that is not VALID, walks no list.  All tasks of the batch have left before any
 // consumer is looked at (phase 2), so a consumer finished in the same batch is never released.
-__global__ void graph_leave_k(u32 n, const u32* __restrict__ task, u32* __restrict__ key, u32* __restrict__ win) {
+// On a sharded graph context the winner is the thread that clears the graph VALID bit, and the owner's key leaves with it.
+template <bool S>
+__global__ void graph_leave_k(u32 n, const u32* __restrict__ task, const GraphKeys k, u32* __restrict__ win) {
     const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const u32 h = task[i];
-    const u32 old = atomicAnd(&key[h], ~(KEY_READY | KEY_VALID | KEY_DONE | KEY_PF));
-    win[i] = (old & KEY_VALID) ? h : GRAPH_NIL;
+    constexpr u32 gone = ~(KEY_READY | KEY_VALID | KEY_DONE | KEY_PF);
+    bool won;
+    if (S) {
+        const u32 b = 1u << (h & 31);
+        won = atomicAnd(&k.gvalid[h >> 5], ~b) & b;
+        if (u32* kh = graph_own<S>(k, h); won && kh) *kh &= gone;
+    } else {
+        won = atomicAnd(&k.key[h], gone) & KEY_VALID;
+    }
+    win[i] = won ? h : GRAPH_NIL;
 }
 
 // the consumer of edge E still waits on the incarnation E was made for
-__device__ __forceinline__ bool graph_edge_waits(const GraphEdge& E, const u32* key, const u32* __restrict__ ggen) {
-    return ggen[E.cons] == E.gen && (key[E.cons] & (KEY_VALID | KEY_READY | KEY_DONE)) == KEY_VALID;
+template <bool S>
+__device__ __forceinline__ bool graph_edge_waits(const GraphEdge& E, const GraphKeys& k, const u32* gdeps, const u32* ggen) {
+    return ggen[E.cons] == E.gen && graph_waiting<S>(k, gdeps, E.cons);
 }
 
 // phase 2: each kept handle walks its consumers; the decrement that reaches zero makes the consumer READY and flags it in the
-// ready bitmap (one bit per handle).  Then the list is emptied.
-__global__ void graph_release_k(u32 n, const u32* __restrict__ win, u32* key, u32* __restrict__ gdeps,
+// ready bitmap (one bit per handle; on a sharded graph context only the handles it owns).  Then the list is emptied.
+template <bool S>
+__global__ void graph_release_k(u32 n, const u32* __restrict__ win, const GraphKeys k, u32* gdeps,
                                 const u32* __restrict__ ggen, u32* __restrict__ ghead, const GraphEdge* __restrict__ pool,
                                 u32* __restrict__ bits) {
     const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -138,9 +203,11 @@ __global__ void graph_release_k(u32 n, const u32* __restrict__ win, u32* key, u3
     if (h == GRAPH_NIL) return;
     for (u32 e = ghead[h]; e != GRAPH_NIL;) {
         const GraphEdge E = pool[e];
-        if (graph_edge_waits(E, key, ggen) && atomicSub(&gdeps[E.cons], 1u) == 1u) {
-            atomicOr(&key[E.cons], KEY_READY);
-            atomicOr(&bits[E.cons >> 5], 1u << (E.cons & 31));
+        if (graph_edge_waits<S>(E, k, gdeps, ggen) && atomicSub(&gdeps[E.cons], 1u) == 1u) {
+            if (u32* kc = graph_own<S>(k, E.cons)) {
+                atomicOr(kc, KEY_READY);
+                atomicOr(&bits[E.cons >> 5], 1u << (E.cons & 31));
+            }
         }
         e = E.next;
     }
@@ -194,14 +261,16 @@ __global__ void graph_unlink_k(u32 n, const u32* __restrict__ task, u32 n_handle
 }
 
 // pool compaction, pass 1: edges whose consumer still waits on their incarnation, per block of 2048 producers
+template <bool S>
 __global__ void __launch_bounds__(GRAPH_NT) graph_gc_count_k(u32 n_handles, const u32* __restrict__ ghead,
-                                                              const GraphEdge* __restrict__ pool, const u32* __restrict__ key,
-                                                              const u32* __restrict__ ggen, u32* __restrict__ blk) {
+                                                              const GraphEdge* __restrict__ pool, const GraphKeys k,
+                                                              const u32* __restrict__ gdeps, const u32* __restrict__ ggen,
+                                                              u32* __restrict__ blk) {
     const u32 h0 = (blockIdx.x * GRAPH_NT + threadIdx.x) * GRAPH_PER_THREAD;
     u32 c = 0;
-    for (u32 k = 0; k < GRAPH_PER_THREAD; ++k) {
-        if (h0 + k >= n_handles) break;
-        for (u32 e = ghead[h0 + k]; e != GRAPH_NIL; e = pool[e].next) c += graph_edge_waits(pool[e], key, ggen) ? 1u : 0u;
+    for (u32 j = 0; j < GRAPH_PER_THREAD; ++j) {
+        if (h0 + j >= n_handles) break;
+        for (u32 e = ghead[h0 + j]; e != GRAPH_NIL; e = pool[e].next) c += graph_edge_waits<S>(pool[e], k, gdeps, ggen) ? 1u : 0u;
     }
     u32 sum;
     graph_block_scan<GRAPH_NT>(c, &sum);
@@ -209,25 +278,26 @@ __global__ void __launch_bounds__(GRAPH_NT) graph_gc_count_k(u32 n_handles, cons
 }
 
 // pass 2 (blk scanned): every list is rewritten, in its order, into consecutive slots of the fresh pool
+template <bool S>
 __global__ void __launch_bounds__(GRAPH_NT) graph_gc_move_k(u32 n_handles, u32* __restrict__ ghead,
                                                              const GraphEdge* __restrict__ pool, GraphEdge* __restrict__ fresh,
-                                                             const u32* __restrict__ key, const u32* __restrict__ ggen,
-                                                             const u32* __restrict__ blk) {
+                                                             const GraphKeys k, const u32* __restrict__ gdeps,
+                                                             const u32* __restrict__ ggen, const u32* __restrict__ blk) {
     const u32 h0 = (blockIdx.x * GRAPH_NT + threadIdx.x) * GRAPH_PER_THREAD;
     u32 c = 0;
-    for (u32 k = 0; k < GRAPH_PER_THREAD; ++k) {
-        if (h0 + k >= n_handles) break;
-        for (u32 e = ghead[h0 + k]; e != GRAPH_NIL; e = pool[e].next) c += graph_edge_waits(pool[e], key, ggen) ? 1u : 0u;
+    for (u32 j = 0; j < GRAPH_PER_THREAD; ++j) {
+        if (h0 + j >= n_handles) break;
+        for (u32 e = ghead[h0 + j]; e != GRAPH_NIL; e = pool[e].next) c += graph_edge_waits<S>(pool[e], k, gdeps, ggen) ? 1u : 0u;
     }
     u32 sum;
     u32 pos = blk[blockIdx.x] + graph_block_scan<GRAPH_NT>(c, &sum);
-    for (u32 k = 0; k < GRAPH_PER_THREAD; ++k) {
-        const u32 h = h0 + k;
+    for (u32 j = 0; j < GRAPH_PER_THREAD; ++j) {
+        const u32 h = h0 + j;
         if (h >= n_handles) break;
         u32 first = GRAPH_NIL, prev = GRAPH_NIL;
         for (u32 e = ghead[h]; e != GRAPH_NIL; e = pool[e].next) {
             const GraphEdge E = pool[e];
-            if (!graph_edge_waits(E, key, ggen)) continue;
+            if (!graph_edge_waits<S>(E, k, gdeps, ggen)) continue;
             fresh[pos] = GraphEdge{E.cons, E.gen, GRAPH_NIL};
             if (prev == GRAPH_NIL) first = pos; else fresh[prev].next = pos;
             prev = pos++;
@@ -236,7 +306,8 @@ __global__ void __launch_bounds__(GRAPH_NT) graph_gc_move_k(u32 n_handles, u32* 
     }
 }
 
-// hqs_graph_debug: out[0] += linked edges, out[1] += waiting tasks (VALID, neither READY nor DONE)
+// hqs_graph_debug: out[0] += linked edges (ghead != nullptr), out[1] += waiting tasks (key != nullptr: VALID, neither READY
+// nor DONE).  A sharded graph context counts the edges over its replicated lists and the waiting tasks over its own keys.
 __global__ void graph_debug_k(u32 n_handles, const u32* __restrict__ key, const u32* __restrict__ ghead,
                               const GraphEdge* __restrict__ pool, unsigned long long* __restrict__ out) {
     const u32 h = blockIdx.x * blockDim.x + threadIdx.x;
@@ -244,7 +315,7 @@ __global__ void graph_debug_k(u32 n_handles, const u32* __restrict__ key, const 
     if (h < n_handles) {
         if (ghead)
             for (u32 e = ghead[h]; e != GRAPH_NIL; e = pool[e].next) ++edges;
-        waiting = (key[h] & (KEY_VALID | KEY_READY | KEY_DONE)) == KEY_VALID ? 1u : 0u;
+        if (key) waiting = (key[h] & (KEY_VALID | KEY_READY | KEY_DONE)) == KEY_VALID ? 1u : 0u;
     }
     edges = __reduce_add_sync(0xffffffffu, edges);
     waiting = __reduce_add_sync(0xffffffffu, waiting);
@@ -267,7 +338,8 @@ struct GraphCancelSync {
 constexpr u32 GRAPH_CANCEL_NT = 256;
 
 // the named handles that are VALID seed the work list (host-checked: every handle < n_handles)
-__global__ void graph_cancel_seed_k(u32 n, const u32* __restrict__ task, const u32* __restrict__ key, u32* __restrict__ bits,
+template <bool S>
+__global__ void graph_cancel_seed_k(u32 n, const u32* __restrict__ task, const GraphKeys k, u32* __restrict__ bits,
                                     u32* __restrict__ work, GraphCancelSync* __restrict__ s) {
     const u32 i = blockIdx.x * blockDim.x + threadIdx.x, lane = threadIdx.x & 31;
     u32 h = GRAPH_NIL;
@@ -275,7 +347,7 @@ __global__ void graph_cancel_seed_k(u32 n, const u32* __restrict__ task, const u
     if (i < n) {
         h = task[i];
         const u32 b = 1u << (h & 31);
-        won = (key[h] & KEY_VALID) && !(atomicOr(&bits[h >> 5], b) & b);      // a handle named twice is admitted once
+        won = graph_valid<S>(k, h) && !(atomicOr(&bits[h >> 5], b) & b);      // a handle named twice is admitted once
     }
     const u32 m = __ballot_sync(0xffffffffu, won);
     if (!m) return;
@@ -326,8 +398,11 @@ __device__ u32 graph_cancel_pop(const u32* work, GraphCancelSync* s) {
 // links, 32 edges at a time, and every lane tests one edge), admits each consumer that still waits on the edge's incarnation
 // and wins its bit, keeps the first one it admits to walk next (a chain never goes through the list) and appends the rest.
 // So the work list holds only part of the closure; the bitmap holds all of it.
-// key, ggen, ghead and pool are only read: nothing leaves the table before graph_cancel_apply_k.
-__global__ void __launch_bounds__(GRAPH_CANCEL_NT) graph_cancel_mark_k(const u32* __restrict__ key, const u32* __restrict__ ggen,
+// The keys, gvalid, gdeps, ggen, ghead and pool are only read: nothing leaves the table before graph_cancel_apply_k.  A
+// sharded graph context marks the whole closure, whichever rank owns its handles.
+template <bool S>
+__global__ void __launch_bounds__(GRAPH_CANCEL_NT) graph_cancel_mark_k(const GraphKeys k, const u32* __restrict__ gdeps,
+                                                                        const u32* __restrict__ ggen,
                                                                         const u32* __restrict__ ghead,
                                                                         const GraphEdge* __restrict__ pool, u32* bits, u32* work,
                                                                         GraphCancelSync* s) {
@@ -358,8 +433,7 @@ __global__ void __launch_bounds__(GRAPH_CANCEL_NT) graph_cancel_mark_k(const u32
             if (lane < cnt) {
                 c = s_cons[w0 + lane];
                 const u32 b = 1u << (c & 31);
-                won = ggen[c] == s_gen[w0 + lane] && (key[c] & (KEY_VALID | KEY_READY | KEY_DONE)) == KEY_VALID &&
-                      !(atomicOr(&bits[c >> 5], b) & b);
+                won = ggen[c] == s_gen[w0 + lane] && graph_waiting<S>(k, gdeps, c) && !(atomicOr(&bits[c >> 5], b) & b);
             }
             __syncwarp();
             u32 m = __ballot_sync(0xffffffffu, won);
@@ -390,15 +464,18 @@ __global__ void __launch_bounds__(GRAPH_CANCEL_NT) graph_cancel_mark_k(const u32
 
 // After the ordered emit (graph_ready_emit_k wrote the marked handles ascending to out[0 .. *n_out) and cleared the bitmap),
 // and only if the marking drained its list: every marked handle leaves the table (as graph_leave_k makes it leave) and its
-// consumer list is emptied.  The work list returns to GRAPH_NIL either way.
+// consumer list is emptied.  The work list returns to GRAPH_NIL either way.  A sharded graph context clears the graph VALID
+// bit of every marked handle and the keys of the ones it owns.
+template <bool S>
 __global__ void graph_cancel_apply_k(u32* __restrict__ work, const GraphCancelSync* __restrict__ s, const u32* __restrict__ out,
-                                     const u32* __restrict__ n_out, u32* __restrict__ key, u32* __restrict__ ghead) {
+                                     const u32* __restrict__ n_out, const GraphKeys k, u32* __restrict__ ghead) {
     const u32 stride = gridDim.x * blockDim.x, i0 = blockIdx.x * blockDim.x + threadIdx.x;
     for (u32 i = i0, n = s->tail; i < n; i += stride) work[i] = GRAPH_NIL;
     if (!s->done || s->error) return;
     for (u32 i = i0, n = *n_out; i < n; i += stride) {
         const u32 h = out[i];
-        key[h] &= ~(KEY_READY | KEY_VALID | KEY_DONE | KEY_PF);
+        if (u32* kh = graph_own<S>(k, h)) *kh &= ~(KEY_READY | KEY_VALID | KEY_DONE | KEY_PF);
+        if (S) atomicAnd(&k.gvalid[h >> 5], ~(1u << (h & 31)));
         ghead[h] = GRAPH_NIL;
     }
 }

@@ -43,6 +43,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <new>
 #include <string>
 #include <numeric>
@@ -131,6 +132,12 @@ struct hqs_ctx {
     std::vector<u32> g_new_ready;       // what *new_ready of hqs_graph_finished / *cancelled of hqs_graph_cancel points to
     u32* d_gwork = nullptr;             // [cap_handles] work list of hqs_graph_cancel's marking (GRAPH_NIL between calls)
     GraphCancelSync* d_gcsync = nullptr;
+    // sharded graph (hqs_shard_graph_init): the graph arrays above are replicated over the global handles [0, g_total) and
+    // keep that size; the key table holds the owned handles [g_lo, g_hi) at h - g_lo
+    bool shard_graph = false;
+    bool shard_graph_failed = false;    // a sharded graph call failed on the device: this replica may differ from the others
+    u32 g_total = 0, g_lo = 0, g_hi = 0;
+    u32* d_gvalid = nullptr;            // [g_total / 32] the graph's VALID bits
     // push staging (device)
     u32* d_push_task = nullptr; u32* d_push_cls = nullptr; u64* d_push_prio = nullptr;
     u32 push_cap = 0;
@@ -227,7 +234,7 @@ int ensure_handles(hqs_ctx* ctx, u32 need) {
     int rc;
     if ((rc = dev_realloc(ctx, &ctx->d_key, ctx->cap_handles, cap, true, true))) return rc;
     if ((rc = dev_realloc(ctx, &ctx->d_prio, ctx->cap_handles, cap, true, true))) return rc;
-    if (ctx->graph_storage) {
+    if (ctx->graph_storage && !ctx->shard_graph) {
         if ((rc = dev_realloc(ctx, &ctx->d_gdeps, ctx->cap_handles, cap, true, true))) return rc;
         if ((rc = dev_realloc(ctx, &ctx->d_ggen, ctx->cap_handles, cap, true, true))) return rc;
         if ((rc = dev_realloc(ctx, &ctx->d_ghead, ctx->cap_handles, cap, true, false))) return rc;
@@ -242,10 +249,11 @@ int ensure_handles(hqs_ctx* ctx, u32 need) {
     return HQS_OK;
 }
 
-// the per-handle graph arrays, at the table's current capacity (ensure_handles grows them from then on)
+// the per-handle graph arrays, at the table's current capacity (ensure_handles grows them from then on), or over the global
+// handles of a sharded graph context
 int ensure_graph_storage(hqs_ctx* ctx) {
     if (ctx->graph_storage) return HQS_OK;
-    const u32 cap = ctx->cap_handles;
+    const u32 cap = ctx->shard_graph ? (ctx->g_total + 1023u) & ~1023u : ctx->cap_handles;
     int rc;
     if (!ctx->d_gsmall) CU(cudaMalloc(&ctx->d_gsmall, 4 * sizeof(u32)));
     if (!ctx->d_gcsync) CU(cudaMalloc(&ctx->d_gcsync, sizeof(GraphCancelSync)));
@@ -1041,7 +1049,7 @@ void hqs_destroy(hqs_ctx* ctx) {
                         ctx->d_seg_wv, ctx->d_out, ctx->d_hdr, ctx->d_free_after, ctx->d_tickin, ctx->d_sync, ctx->d_pk_fr,
                         ctx->d_pk_quota, ctx->d_pk_taken, ctx->d_pk_cand, ctx->d_pk_meta, ctx->d_prune_lv, ctx->d_prune_live,
                         ctx->d_gdeps, ctx->d_ggen, ctx->d_ghead, ctx->d_gbits, ctx->d_gready, ctx->d_gblk, ctx->d_gsmall,
-                        ctx->d_pool, ctx->d_gstage, ctx->d_gwork, ctx->d_gcsync};
+                        ctx->d_pool, ctx->d_gstage, ctx->d_gwork, ctx->d_gcsync, ctx->d_gvalid};
     for (void* p : dev_ptrs) if (p) cudaFree(p);
     for (void* p : ctx->x_opened) cudaIpcCloseMemHandle(p);
     if (ctx->d_xbuf) cudaFree(ctx->d_xbuf);
@@ -1153,27 +1161,44 @@ int hqs_classes_set(hqs_ctx* ctx, uint32_t n_classes, const hqs_class* classes) 
 
 namespace {
 // The dependencies of a graph push, staged by hqs_graph_push: d_gstage = dependency offsets [n + 1], then the dependency
-// handles; the counted edges take the pool slots e0 + j.
+// handles; the counted edges take the pool slots e0 + j.  task: the batch's n handles on the device on a sharded graph
+// context (global; push_impl's own arrays are the owned part of the batch only); nullptr: push_impl's staged handles.
 struct GraphBatch {
     u32 e0;
+    u32 n;
+    const u32* task;
 };
+
+// how the graph kernels see this context's keys (hqs_graph.cuh)
+GraphKeys graph_keys(const hqs_ctx* ctx) {
+    if (!ctx->shard_graph) return GraphKeys{ctx->d_key, nullptr, 0u, ~0u};
+    return GraphKeys{ctx->d_key, ctx->d_gvalid, ctx->g_lo, ctx->g_lo + std::min(ctx->cap_handles, ctx->g_hi - ctx->g_lo)};
+}
+
+// the handles the graph calls accept: the table of one context, the global range of a sharded graph context
+u32 graph_bound(const hqs_ctx* ctx) { return ctx->shard_graph ? ctx->g_total : ctx->n_handles; }
 
 // shared body of hqs_ready_push / hqs_ready_push_range (task == nullptr: handles first_handle .. first_handle + n - 1) and
 // hqs_graph_push (g != nullptr: the batch is also rejected if a pushed handle is VALID, and graph_link_k runs after push_k;
-// h_small[2] receives the number of tasks ready at once)
+// h_small[2] receives the number of tasks ready at once).  A sharded graph push passes the owned part of its batch, which
+// may be empty.
 int push_impl(hqs_ctx* ctx, u32 n, const u32* task, u32 first_handle, const u32* class_id, const u64* priority,
               const GraphBatch* g = nullptr) {
     if (ctx->Q == 0) return fail(ctx, HQS_E_STATE, "hqs_classes_set has not been called");
     if (ctx->dag) return fail(ctx, HQS_E_STATE, "hqs_ready_push is not available after hqs_dag_load");
+    if (!g && ctx->shard_graph)
+        return fail(ctx, HQS_E_STATE, "hqs_ready_push is not available on a sharded graph context (hqs_shard_graph_push)");
     CU(cudaSetDevice(ctx->device));
     if (int rc_ = ensure_push_staging(ctx, n)) return rc_;
-    if (task) CU(cudaMemcpyAsync(ctx->d_push_task, task, (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream));
-    CU(cudaMemcpyAsync(ctx->d_push_cls, class_id, (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream));
-    CU(cudaMemcpyAsync(ctx->d_push_prio, priority, (size_t)n * 8, cudaMemcpyHostToDevice, ctx->stream));
+    if (n) {
+        if (task) CU(cudaMemcpyAsync(ctx->d_push_task, task, (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream));
+        CU(cudaMemcpyAsync(ctx->d_push_cls, class_id, (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream));
+        CU(cudaMemcpyAsync(ctx->d_push_prio, priority, (size_t)n * 8, cudaMemcpyHostToDevice, ctx->stream));
+    }
     // the table must hold the largest handle before the kernel runs: a host pass over the handle array while the staging
     // copies are in flight (a range push knows it); class ids are validated on the device (push_validate_k)
-    u32 max_h = first_handle + (n - 1);
-    if (task) {
+    u32 max_h = n ? first_handle + (n - 1) : 0u;
+    if (task && n) {
         u32 dummy = 0;
         max_of_u32_pair(task, task, n, &max_h, &dummy);
     } else if (max_h < first_handle) {
@@ -1183,20 +1208,33 @@ int push_impl(hqs_ctx* ctx, u32 n, const u32* task, u32 first_handle, const u32*
         cudaStreamSynchronize(ctx->stream);      // the caller may free its arrays as soon as we return
         return fail(ctx, HQS_E_INVALID, "task handle 0xFFFFFFFF is reserved");
     }
-    int rc = ensure_handles(ctx, max_h + 1);
+    int rc = n ? ensure_handles(ctx, max_h + 1) : HQS_OK;
     if (rc) { cudaStreamSynchronize(ctx->stream); return rc; }
     CU(cudaMemsetAsync(ctx->d_newcnt, 0, 2 * sizeof(u32), ctx->stream));
-    push_validate_k<<<(n + 255) / 256, 256, 0, ctx->stream>>>(n, ctx->d_push_cls, ctx->Q, ctx->d_newcnt);
-    if (g) graph_validate_k<<<(n + 255) / 256, 256, 0, ctx->stream>>>(n, ctx->d_push_task, ctx->d_key, ctx->n_handles, ctx->d_newcnt);
-    push_k<<<(n + 255) / 256, 256, 0, ctx->stream>>>(n, task ? ctx->d_push_task : nullptr, first_handle, ctx->d_push_cls,
-                                                     ctx->d_push_prio, ctx->d_key, ctx->d_prio, ctx->d_levels,
-                                                     (u32)ctx->dev_levels.size(), ctx->coarse ? 1 : 0, ctx->d_newcnt, ctx->d_newprio);
-    ctx->stats.kernel_launches += 2;
+    const GraphKeys gk = graph_keys(ctx);
+    const u32* gtask = g && g->task ? g->task : ctx->d_push_task;     // after ensure_push_staging, which may move it
+    if (n) push_validate_k<<<(n + 255) / 256, 256, 0, ctx->stream>>>(n, ctx->d_push_cls, ctx->Q, ctx->d_newcnt);
+    if (g)
+        graph_dispatch(ctx->shard_graph, [&](auto S) {
+            graph_validate_k<decltype(S)::value><<<(g->n + 255) / 256, 256, 0, ctx->stream>>>(g->n, gtask, gk, graph_bound(ctx),
+                                                                                             ctx->d_newcnt);
+        });
+    if (n)
+        push_k<<<(n + 255) / 256, 256, 0, ctx->stream>>>(n, task ? ctx->d_push_task : nullptr, first_handle, ctx->d_push_cls,
+                                                         ctx->d_push_prio, ctx->d_key, ctx->d_prio, ctx->d_levels,
+                                                         (u32)ctx->dev_levels.size(), ctx->coarse ? 1 : 0, ctx->d_newcnt, ctx->d_newprio);
+    ctx->stats.kernel_launches += n ? 2 : 0;
     if (g) {
         CU(cudaMemsetAsync(ctx->d_gsmall, 0, sizeof(u32), ctx->stream));
-        graph_link_k<<<(n + 255) / 256, 256, 0, ctx->stream>>>(n, ctx->d_push_task, ctx->d_gstage, ctx->d_gstage + n + 1, g->e0,
-                                                               ctx->d_newcnt, ctx->d_key, ctx->d_gdeps, ctx->d_ggen, ctx->d_ghead,
-                                                               ctx->d_pool, ctx->d_gsmall);
+        if (ctx->shard_graph) {
+            graph_enter_k<<<(g->n + 255) / 256, 256, 0, ctx->stream>>>(g->n, gtask, ctx->d_newcnt, ctx->d_gvalid);
+            ctx->stats.kernel_launches++;
+        }
+        graph_dispatch(ctx->shard_graph, [&](auto S) {
+            graph_link_k<decltype(S)::value><<<(g->n + 255) / 256, 256, 0, ctx->stream>>>(
+                g->n, gtask, ctx->d_gstage, ctx->d_gstage + g->n + 1, g->e0, ctx->d_newcnt, gk, ctx->d_gdeps, ctx->d_ggen,
+                ctx->d_ghead, ctx->d_pool, ctx->d_gsmall);
+        });
         CU(cudaMemcpyAsync(ctx->h_small + 2, ctx->d_gsmall, sizeof(u32), cudaMemcpyDeviceToHost, ctx->stream));
         ctx->stats.kernel_launches += 2;
     }
@@ -1210,7 +1248,7 @@ int push_impl(hqs_ctx* ctx, u32 n, const u32* task, u32 first_handle, const u32*
     CU(cudaStreamSynchronize(ctx->stream));
     if (ctx->h_small[1] & 1u) return fail(ctx, HQS_E_INVALID, "a class id of the batch is >= n_classes %u (nothing was pushed)", ctx->Q);
     if (ctx->h_small[1]) return fail(ctx, HQS_E_INVALID, "a handle of the batch is a live task (nothing was pushed)");
-    ctx->n_handles = std::max(ctx->n_handles, max_h + 1);
+    if (n) ctx->n_handles = std::max(ctx->n_handles, max_h + 1);
     ctx->stats.n_handles = ctx->n_handles;
     const u32 newcnt = ctx->h_small[0];
     bool grew = false;
@@ -1313,6 +1351,8 @@ int hqs_ready_remove(hqs_ctx* ctx, uint32_t n, const uint32_t* task) {
     if (!ctx) return HQS_E_INVALID;
     if (n == 0) return HQS_OK;
     if (!task) return fail(ctx, HQS_E_INVALID, "null task array");
+    if (ctx->shard_graph)
+        return fail(ctx, HQS_E_STATE, "hqs_ready_remove is not available on a sharded graph context (hqs_shard_graph_remove)");
     CU(cudaSetDevice(ctx->device));
     if (int rc_ = ensure_push_staging(ctx, n)) return rc_;
     CU(cudaMemcpyAsync(ctx->d_push_task, task, (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream));
@@ -1371,6 +1411,7 @@ int hqs_dag_load(hqs_ctx* ctx, uint32_t n_tasks, const uint32_t* class_id, const
     if (!n_tasks || !class_id || !priority || !n_deps || !cons_off) return fail(ctx, HQS_E_INVALID, "null DAG arrays");
     if (ctx->Q == 0) return fail(ctx, HQS_E_STATE, "hqs_classes_set has not been called");
     if (ctx->graph) return fail(ctx, HQS_E_STATE, "hqs_dag_load is not available after hqs_graph_push");
+    if (ctx->shard_graph) return fail(ctx, HQS_E_STATE, "hqs_dag_load is not available on a sharded graph context");
     const u32 n_edges = cons_off[n_tasks];
     if (n_edges && !cons) return fail(ctx, HQS_E_INVALID, "null consumer array");
     for (u32 i = 0; i < n_tasks; ++i)
@@ -1442,17 +1483,59 @@ namespace {
 int graph_mode_check(hqs_ctx* ctx, const char* what) {
     if (ctx->dag) return fail(ctx, HQS_E_STATE, "%s is not available after hqs_dag_load", what);
     if (ctx->x_world) return fail(ctx, HQS_E_STATE, "%s is not available on a sharded ready set", what);
+    if (ctx->shard_graph) return fail(ctx, HQS_E_STATE, "%s is not available on a sharded graph context (hqs_shard_graph_*)", what);
     if (ctx->tick_pending) return fail(ctx, HQS_E_STATE, "the previous tick has not been fetched");
+    return HQS_OK;
+}
+
+// ... and the states in which the sharded graph calls are refused
+int shard_graph_mode_check(hqs_ctx* ctx, const char* what) {
+    if (!ctx->shard_graph) return fail(ctx, HQS_E_STATE, "%s needs hqs_shard_graph_init", what);
+    if (ctx->shard_graph_failed)
+        return fail(ctx, HQS_E_STATE, "%s: an earlier sharded graph call failed on the device, so this rank's replica may differ "
+                    "from the others; the sharded graph must be set up again on new contexts", what);
+    if (ctx->tick_pending) return fail(ctx, HQS_E_STATE, "the previous tick has not been fetched");
+    return HQS_OK;
+}
+
+// A sharded graph call that failed on the device (HQS_E_CUDA: a CUDA error, an allocation, the cancel marking's time-out) may
+// have changed this rank's replica and not the others', or the others' and not this one: the context refuses the sharded
+// graph calls from then on.  The other failures are decided alike on every rank from the same arguments and change nothing.
+int shard_graph_outcome(hqs_ctx* ctx, int rc) {
+    if (rc == HQS_E_CUDA) ctx->shard_graph_failed = true;
+    return rc;
+}
+
+// the body of hqs_shard_graph_remove, after the mode check
+int shard_graph_remove_impl(hqs_ctx* ctx, u32 n, const u32* task) {
+    if (n == 0) return HQS_OK;
+    if (!task) return fail(ctx, HQS_E_INVALID, "null task array");
+    for (u32 i = 0; i < n; ++i)
+        if (task[i] >= ctx->g_total)
+            return fail(ctx, HQS_E_INVALID, "task %u >= n_total %u (nothing was removed)", task[i], ctx->g_total);
+    CU(cudaSetDevice(ctx->device));
+    if (int rc = ensure_push_staging(ctx, n)) return rc;
+    CU(cudaMemcpyAsync(ctx->d_push_task, task, (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream));
+    // what hqs_ready_remove does, over the replica: the owner's keys and every rank's graph VALID bits and consumer lists go
+    graph_leave_k<true><<<(n + 255) / 256, 256, 0, ctx->stream>>>(n, ctx->d_push_task, graph_keys(ctx), ctx->d_push_cls);
+    graph_unlink_k<<<(n + 255) / 256, 256, 0, ctx->stream>>>(n, ctx->d_push_task, ctx->g_total, ctx->d_ghead);
+    ctx->stats.kernel_launches += 2;
+    CU(cudaGetLastError());
+    CU(cudaStreamSynchronize(ctx->stream));
     return HQS_OK;
 }
 
 // Before a push whose edges do not fit: the pool keeps only the edges whose consumer still waits on their incarnation,
 // rewritten list by list into a fresh pool of max(capacity, 2 * live + n_edges) slots.
 int graph_compact(hqs_ctx* ctx, u32 n_edges) {
-    const u32 nb = (ctx->n_handles + GRAPH_PER_BLOCK - 1) / GRAPH_PER_BLOCK;
+    const u32 nh = graph_bound(ctx), nb = (nh + GRAPH_PER_BLOCK - 1) / GRAPH_PER_BLOCK;
+    const GraphKeys gk = graph_keys(ctx);
     u32 live = 0;
     if (nb) {
-        graph_gc_count_k<<<nb, GRAPH_NT, 0, ctx->stream>>>(ctx->n_handles, ctx->d_ghead, ctx->d_pool, ctx->d_key, ctx->d_ggen, ctx->d_gblk);
+        graph_dispatch(ctx->shard_graph, [&](auto S) {
+            graph_gc_count_k<decltype(S)::value><<<nb, GRAPH_NT, 0, ctx->stream>>>(nh, ctx->d_ghead, ctx->d_pool, gk, ctx->d_gdeps,
+                                                                                  ctx->d_ggen, ctx->d_gblk);
+        });
         graph_scan_k<<<1, 1024, 0, ctx->stream>>>(nb, ctx->d_gblk, ctx->d_gsmall + 2);
         ctx->stats.kernel_launches += 2;
         CU(cudaGetLastError());
@@ -1465,7 +1548,10 @@ int graph_compact(hqs_ctx* ctx, u32 n_edges) {
     GraphEdge* fresh = nullptr;
     CU(cudaMalloc(&fresh, (size_t)want * sizeof(GraphEdge)));
     if (nb) {
-        graph_gc_move_k<<<nb, GRAPH_NT, 0, ctx->stream>>>(ctx->n_handles, ctx->d_ghead, ctx->d_pool, fresh, ctx->d_key, ctx->d_ggen, ctx->d_gblk);
+        graph_dispatch(ctx->shard_graph, [&](auto S) {
+            graph_gc_move_k<decltype(S)::value><<<nb, GRAPH_NT, 0, ctx->stream>>>(nh, ctx->d_ghead, ctx->d_pool, fresh, gk,
+                                                                                 ctx->d_gdeps, ctx->d_ggen, ctx->d_gblk);
+        });
         ctx->stats.kernel_launches++;
         CU(cudaGetLastError());
     }
@@ -1478,15 +1564,22 @@ int graph_compact(hqs_ctx* ctx, u32 n_edges) {
     return HQS_OK;
 }
 
-// the device half of hqs_graph_push's validation on its own, before a compaction (a rejected batch changes nothing)
-int graph_prevalidate(hqs_ctx* ctx, u32 n, const u32* task, const u32* class_id) {
+// the device half of hqs_graph_push's validation on its own, before a compaction (a rejected batch changes nothing).  A
+// sharded graph push has checked its class ids on the host and staged its handles at d_task.
+int graph_prevalidate(hqs_ctx* ctx, u32 n, const u32* task, const u32* class_id, const u32* d_task) {
     if (int rc = ensure_push_staging(ctx, n)) return rc;
-    CU(cudaMemcpyAsync(ctx->d_push_task, task, (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream));
-    CU(cudaMemcpyAsync(ctx->d_push_cls, class_id, (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream));
     CU(cudaMemsetAsync(ctx->d_newcnt, 0, 2 * sizeof(u32), ctx->stream));
-    push_validate_k<<<(n + 255) / 256, 256, 0, ctx->stream>>>(n, ctx->d_push_cls, ctx->Q, ctx->d_newcnt);
-    graph_validate_k<<<(n + 255) / 256, 256, 0, ctx->stream>>>(n, ctx->d_push_task, ctx->d_key, ctx->n_handles, ctx->d_newcnt);
-    ctx->stats.kernel_launches += 2;
+    if (ctx->shard_graph) {
+        graph_validate_k<true><<<(n + 255) / 256, 256, 0, ctx->stream>>>(n, d_task, graph_keys(ctx), ctx->g_total, ctx->d_newcnt);
+        ctx->stats.kernel_launches++;
+    } else {
+        CU(cudaMemcpyAsync(ctx->d_push_task, task, (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream));
+        CU(cudaMemcpyAsync(ctx->d_push_cls, class_id, (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream));
+        push_validate_k<<<(n + 255) / 256, 256, 0, ctx->stream>>>(n, ctx->d_push_cls, ctx->Q, ctx->d_newcnt);
+        graph_validate_k<false><<<(n + 255) / 256, 256, 0, ctx->stream>>>(n, ctx->d_push_task, graph_keys(ctx), ctx->n_handles,
+                                                                          ctx->d_newcnt);
+        ctx->stats.kernel_launches += 2;
+    }
     CU(cudaGetLastError());
     CU(cudaMemcpyAsync(ctx->h_small, ctx->d_newcnt, 2 * sizeof(u32), cudaMemcpyDeviceToHost, ctx->stream));
     CU(cudaStreamSynchronize(ctx->stream));
@@ -1507,18 +1600,15 @@ bool has_duplicate(const u32* d, u32 k, std::vector<u32>& scratch) {
     std::sort(scratch.begin(), scratch.end());
     return std::adjacent_find(scratch.begin(), scratch.end()) != scratch.end();
 }
-}  // namespace
-
-extern "C" {
-
-int hqs_graph_push(hqs_ctx* ctx, uint32_t n, const uint32_t* task, const uint32_t* class_id, const uint64_t* priority,
-                   const uint32_t* dep_off, const uint32_t* deps, uint32_t* n_ready) {
-    if (!ctx) return HQS_E_INVALID;
-    if (n_ready) *n_ready = 0;
-    if (int rc = graph_mode_check(ctx, "hqs_graph_push")) return rc;
+// The body of hqs_graph_push and hqs_shard_graph_push, after the mode check.  On a sharded graph context the handles are
+// global: every rank checks and links the whole batch, and pushes the keys of the handles it owns.
+int graph_push_impl(hqs_ctx* ctx, u32 n, const u32* task, const u32* class_id, const u64* priority, const u32* dep_off,
+                    const u32* deps, u32* n_ready) {
     if (n == 0) return HQS_OK;
     if (!task || !class_id || !priority || !dep_off) return fail(ctx, HQS_E_INVALID, "null task arrays");
     if (ctx->Q == 0) return fail(ctx, HQS_E_STATE, "hqs_classes_set has not been called");
+    const bool shard = ctx->shard_graph;
+    const u32 bound = graph_bound(ctx);
     // host-knowable checks, then the batch's own dependency lists: the handle -> batch position map is a range test when
     // the handles are consecutive (a job's tasks), a sorted table otherwise
     if (dep_off[0] != 0) return fail(ctx, HQS_E_INVALID, "dep_off[0] = %u, not 0", dep_off[0]);
@@ -1529,7 +1619,19 @@ int hqs_graph_push(hqs_ctx* ctx, uint32_t n, const uint32_t* task, const uint32_
     bool range = true;
     for (u32 i = 0; i < n; ++i) {
         if (task[i] == GRAPH_NIL) return fail(ctx, HQS_E_INVALID, "task handle 0xFFFFFFFF is reserved");
+        if (shard && task[i] >= bound) return fail(ctx, HQS_E_INVALID, "task %u >= n_total %u (nothing was pushed)", task[i], bound);
         range &= task[i] == task[0] + i;
+    }
+    if (shard) {
+        // every rank must see the same rejections and number the levels alike: class ids here, declared priorities only
+        for (u32 i = 0; i < n; ++i)
+            if (class_id[i] >= ctx->Q) return fail(ctx, HQS_E_INVALID, "a class id of the batch is >= n_classes %u (nothing was pushed)", ctx->Q);
+        std::vector<u64> pr;
+        distinct_priorities(priority, n, pr);
+        for (u64 p : pr)
+            if (!std::binary_search(ctx->levels.begin(), ctx->levels.end(), p, std::greater<u64>()))
+                return fail(ctx, HQS_E_INVALID, "priority %llu was not declared with hqs_levels_add (nothing was pushed)",
+                            (unsigned long long)p);
     }
     std::vector<std::pair<u32, u32>>& pos = ctx->g_pos;
     if (!range) {
@@ -1559,7 +1661,7 @@ int hqs_graph_push(hqs_ctx* ctx, uint32_t n, const uint32_t* task, const uint32_
             if (d == task[i]) return fail(ctx, HQS_E_INVALID, "task %u depends on itself", d);
             const u32 p = batch_pos(d);
             if (p == GRAPH_NIL) {
-                if (d >= ctx->n_handles) return fail(ctx, HQS_E_INVALID, "dependency %u of task %u is unknown", d, task[i]);
+                if (d >= bound) return fail(ctx, HQS_E_INVALID, "dependency %u of task %u is unknown", d, task[i]);
                 dep.push_back(d);                // counts if VALID on the device
             } else if (p < i) {
                 dep.push_back(d);                // an earlier task of the batch
@@ -1571,9 +1673,24 @@ int hqs_graph_push(hqs_ctx* ctx, uint32_t n, const uint32_t* task, const uint32_
     CU(cudaSetDevice(ctx->device));
     int rc;
     if ((rc = ensure_graph_storage(ctx))) return rc;
+    // d_gstage: offsets, dependencies, then (sharded) the batch's global handles
+    const size_t stage = (size_t)n + 1 + me + (shard ? n : 0);
+    if (stage > ctx->gstage_cap) {
+        const size_t cap = std::max<size_t>(stage * 2, 1u << 16);
+        if ((rc = dev_realloc(ctx, &ctx->d_gstage, 0, cap, false, false))) return rc;
+        ctx->gstage_cap = cap;
+    }
+    // pageable sources: staged by the runtime before the calls return
+    CU(cudaMemcpyAsync(ctx->d_gstage, off.data(), ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, ctx->stream));
+    if (me) CU(cudaMemcpyAsync(ctx->d_gstage + n + 1, dep.data(), (size_t)me * 4, cudaMemcpyHostToDevice, ctx->stream));
+    u32* d_task = nullptr;
+    if (shard) {
+        d_task = ctx->d_gstage + n + 1 + me;
+        CU(cudaMemcpyAsync(d_task, task, (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream));
+    }
     // a push that allocates or compacts the pool is validated on the device first, so that a rejected batch changes nothing
     if (!ctx->d_pool || (u64)ctx->pool_used + me > ctx->pool_cap)
-        if ((rc = graph_prevalidate(ctx, n, task, class_id))) return rc;
+        if ((rc = graph_prevalidate(ctx, n, task, class_id, d_task))) return rc;
     if (!ctx->d_pool) {
         const u64 cap = std::max<u64>(2ull * me, GRAPH_POOL_MIN);
         if (cap >= GRAPH_NIL) return fail(ctx, HQS_E_LIMIT, "the edge pool would need %llu slots", (unsigned long long)cap);
@@ -1583,46 +1700,58 @@ int hqs_graph_push(hqs_ctx* ctx, uint32_t n, const uint32_t* task, const uint32_
     } else if ((u64)ctx->pool_used + me > ctx->pool_cap) {
         if ((rc = graph_compact(ctx, me))) return rc;
     }
-    const size_t stage = (size_t)n + 1 + me;
-    if (stage > ctx->gstage_cap) {
-        const size_t cap = std::max<size_t>(stage * 2, 1u << 16);
-        if ((rc = dev_realloc(ctx, &ctx->d_gstage, 0, cap, false, false))) return rc;
-        ctx->gstage_cap = cap;
+    const GraphBatch g{ctx->pool_used, n, d_task};
+    if (shard) {
+        // the owned part of the batch, as local handles
+        std::vector<u32> ot, oc;
+        std::vector<u64> op;
+        for (u32 i = 0; i < n; ++i)
+            if (task[i] >= ctx->g_lo && task[i] < ctx->g_hi) {
+                ot.push_back(task[i] - ctx->g_lo);
+                oc.push_back(class_id[i]);
+                op.push_back(priority[i]);
+            }
+        rc = push_impl(ctx, (u32)ot.size(), ot.data(), 0, oc.data(), op.data(), &g);
+    } else {
+        rc = push_impl(ctx, n, task, 0, class_id, priority, &g);
     }
-    // pageable sources: staged by the runtime before the calls return
-    CU(cudaMemcpyAsync(ctx->d_gstage, off.data(), ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, ctx->stream));
-    if (me) CU(cudaMemcpyAsync(ctx->d_gstage + n + 1, dep.data(), (size_t)me * 4, cudaMemcpyHostToDevice, ctx->stream));
-    const GraphBatch g{ctx->pool_used};
-    if ((rc = push_impl(ctx, n, task, 0, class_id, priority, &g))) return rc;
+    if (rc) return rc;
     ctx->pool_used += me;
     ctx->graph = true;
     if (n_ready) *n_ready = ctx->h_small[2];
     return HQS_OK;
 }
 
-int hqs_graph_finished(hqs_ctx* ctx, uint32_t n, const uint32_t* task, const uint32_t** new_ready, uint32_t* n_new_ready) {
-    if (!ctx) return HQS_E_INVALID;
-    ctx->g_new_ready.clear();
-    if (new_ready) *new_ready = ctx->g_new_ready.data();
-    if (n_new_ready) *n_new_ready = 0;
-    if (int rc = graph_mode_check(ctx, "hqs_graph_finished")) return rc;
+// The newly ready (hqs_graph_finished) or cancelled (hqs_graph_cancel) handles flagged in d_gbits, ascending, into
+// d_gready; *n into d_gsmall[1].  The bitmap is cleared.
+void graph_emit_bits(hqs_ctx* ctx) {
+    const u32 n_words = (graph_bound(ctx) + 31) / 32, nb = (n_words + GRAPH_PER_BLOCK - 1) / GRAPH_PER_BLOCK;
+    graph_ready_count_k<<<nb, GRAPH_NT, 0, ctx->stream>>>(n_words, ctx->d_gbits, ctx->d_gblk);
+    graph_scan_k<<<1, 1024, 0, ctx->stream>>>(nb, ctx->d_gblk, ctx->d_gsmall + 1);
+    graph_ready_emit_k<<<nb, GRAPH_NT, 0, ctx->stream>>>(n_words, ctx->d_gbits, ctx->d_gblk, ctx->d_gready);
+}
+
+// the body of hqs_graph_finished and hqs_shard_graph_finished, after the mode check
+int graph_finished_impl(hqs_ctx* ctx, u32 n, const u32* task, const u32** new_ready, u32* n_new_ready) {
     if (n == 0) return HQS_OK;
     if (!task) return fail(ctx, HQS_E_INVALID, "null task array");
+    const u32 bound = graph_bound(ctx);
     for (u32 i = 0; i < n; ++i)
-        if (task[i] >= ctx->n_handles) return fail(ctx, HQS_E_INVALID, "task %u >= n_handles %u (nothing was finished)", task[i], ctx->n_handles);
+        if (task[i] >= bound) return fail(ctx, HQS_E_INVALID, "task %u >= n_handles %u (nothing was finished)", task[i], bound);
     CU(cudaSetDevice(ctx->device));
     int rc;
     if ((rc = ensure_graph_storage(ctx))) return rc;
     if ((rc = ensure_push_staging(ctx, n))) return rc;
     u32* win = ctx->d_push_cls;          // the staging of class ids is free during this call
     CU(cudaMemcpyAsync(ctx->d_push_task, task, (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream));
-    graph_leave_k<<<(n + 255) / 256, 256, 0, ctx->stream>>>(n, ctx->d_push_task, ctx->d_key, win);
-    graph_release_k<<<(n + 255) / 256, 256, 0, ctx->stream>>>(n, win, ctx->d_key, ctx->d_gdeps, ctx->d_ggen, ctx->d_ghead,
-                                                              ctx->d_pool, ctx->d_gbits);
-    const u32 n_words = (ctx->n_handles + 31) / 32, nb = (n_words + GRAPH_PER_BLOCK - 1) / GRAPH_PER_BLOCK;
-    graph_ready_count_k<<<nb, GRAPH_NT, 0, ctx->stream>>>(n_words, ctx->d_gbits, ctx->d_gblk);
-    graph_scan_k<<<1, 1024, 0, ctx->stream>>>(nb, ctx->d_gblk, ctx->d_gsmall + 1);
-    graph_ready_emit_k<<<nb, GRAPH_NT, 0, ctx->stream>>>(n_words, ctx->d_gbits, ctx->d_gblk, ctx->d_gready);
+    const GraphKeys gk = graph_keys(ctx);
+    graph_dispatch(ctx->shard_graph, [&](auto S) {
+        constexpr bool s = decltype(S)::value;
+        graph_leave_k<s><<<(n + 255) / 256, 256, 0, ctx->stream>>>(n, ctx->d_push_task, gk, win);
+        graph_release_k<s><<<(n + 255) / 256, 256, 0, ctx->stream>>>(n, win, gk, ctx->d_gdeps, ctx->d_ggen, ctx->d_ghead,
+                                                                     ctx->d_pool, ctx->d_gbits);
+    });
+    graph_emit_bits(ctx);
     ctx->stats.kernel_launches += 5;
     CU(cudaGetLastError());
     CU(cudaMemcpyAsync(ctx->h_small + 3, ctx->d_gsmall + 1, sizeof(u32), cudaMemcpyDeviceToHost, ctx->stream));
@@ -1638,16 +1767,14 @@ int hqs_graph_finished(hqs_ctx* ctx, uint32_t n, const uint32_t* task, const uin
     return HQS_OK;
 }
 
-int hqs_graph_cancel(hqs_ctx* ctx, uint32_t n, const uint32_t* task, const uint32_t** cancelled, uint32_t* n_cancelled) {
-    if (!ctx) return HQS_E_INVALID;
-    ctx->g_new_ready.clear();
-    if (cancelled) *cancelled = ctx->g_new_ready.data();
-    if (n_cancelled) *n_cancelled = 0;
-    if (int rc = graph_mode_check(ctx, "hqs_graph_cancel")) return rc;
+// the body of hqs_graph_cancel and hqs_shard_graph_cancel, after the mode check.  A sharded graph context marks, emits and
+// applies the whole closure and returns the part it owns.
+int graph_cancel_impl(hqs_ctx* ctx, u32 n, const u32* task, const u32** cancelled, u32* n_cancelled) {
     if (n == 0) return HQS_OK;
     if (!task) return fail(ctx, HQS_E_INVALID, "null task array");
+    const u32 bound = graph_bound(ctx);
     for (u32 i = 0; i < n; ++i)
-        if (task[i] >= ctx->n_handles) return fail(ctx, HQS_E_INVALID, "task %u >= n_handles %u (nothing was cancelled)", task[i], ctx->n_handles);
+        if (task[i] >= bound) return fail(ctx, HQS_E_INVALID, "task %u >= n_handles %u (nothing was cancelled)", task[i], bound);
     CU(cudaSetDevice(ctx->device));
     int rc;
     if ((rc = ensure_graph_storage(ctx))) return rc;
@@ -1655,22 +1782,25 @@ int hqs_graph_cancel(hqs_ctx* ctx, uint32_t n, const uint32_t* task, const uint3
     CU(cudaMemcpyAsync(ctx->d_push_task, task, (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream));
     CU(cudaMemsetAsync(ctx->d_gcsync, 0, sizeof(GraphCancelSync), ctx->stream));
     // the launches do not depend on the depth of the closure: seed, marking (the whole closure), ordered emit, apply
-    graph_cancel_seed_k<<<(n + 255) / 256, 256, 0, ctx->stream>>>(n, ctx->d_push_task, ctx->d_key, ctx->d_gbits, ctx->d_gwork,
-                                                                  ctx->d_gcsync);
-    {
-        const u32* key = ctx->d_key; const u32* ggen = ctx->d_ggen; const u32* ghead = ctx->d_ghead;
+    GraphKeys gk = graph_keys(ctx);
+    cudaError_t launched = cudaSuccess;
+    graph_dispatch(ctx->shard_graph, [&](auto S) {
+        constexpr bool s = decltype(S)::value;
+        graph_cancel_seed_k<s><<<(n + 255) / 256, 256, 0, ctx->stream>>>(n, ctx->d_push_task, gk, ctx->d_gbits, ctx->d_gwork,
+                                                                         ctx->d_gcsync);
+        const u32* gdeps = ctx->d_gdeps; const u32* ggen = ctx->d_ggen; const u32* ghead = ctx->d_ghead;
         const GraphEdge* pool = ctx->d_pool;
         u32* bits = ctx->d_gbits; u32* work = ctx->d_gwork; GraphCancelSync* sync = ctx->d_gcsync;
-        void* kargs[] = {&key, &ggen, &ghead, &pool, &bits, &work, &sync};
-        CU(cudaLaunchCooperativeKernel((const void*)graph_cancel_mark_k, dim3(ctx->grid_ctas), dim3(GRAPH_CANCEL_NT), kargs, 0,
-                                       ctx->stream));
-    }
-    const u32 n_words = (ctx->n_handles + 31) / 32, nb = (n_words + GRAPH_PER_BLOCK - 1) / GRAPH_PER_BLOCK;
-    graph_ready_count_k<<<nb, GRAPH_NT, 0, ctx->stream>>>(n_words, ctx->d_gbits, ctx->d_gblk);
-    graph_scan_k<<<1, 1024, 0, ctx->stream>>>(nb, ctx->d_gblk, ctx->d_gsmall + 1);
-    graph_ready_emit_k<<<nb, GRAPH_NT, 0, ctx->stream>>>(n_words, ctx->d_gbits, ctx->d_gblk, ctx->d_gready);
-    graph_cancel_apply_k<<<ctx->sm_count * 4, 256, 0, ctx->stream>>>(ctx->d_gwork, ctx->d_gcsync, ctx->d_gready, ctx->d_gsmall + 1,
-                                                                     ctx->d_key, ctx->d_ghead);
+        void* kargs[] = {&gk, &gdeps, &ggen, &ghead, &pool, &bits, &work, &sync};
+        launched = cudaLaunchCooperativeKernel((const void*)graph_cancel_mark_k<s>, dim3(ctx->grid_ctas), dim3(GRAPH_CANCEL_NT),
+                                               kargs, 0, ctx->stream);
+    });
+    CU(launched);
+    graph_emit_bits(ctx);
+    graph_dispatch(ctx->shard_graph, [&](auto S) {
+        graph_cancel_apply_k<decltype(S)::value><<<ctx->sm_count * 4, 256, 0, ctx->stream>>>(
+            ctx->d_gwork, ctx->d_gcsync, ctx->d_gready, ctx->d_gsmall + 1, gk, ctx->d_ghead);
+    });
     ctx->stats.kernel_launches += 6;
     CU(cudaGetLastError());
     GraphCancelSync hs;
@@ -1686,20 +1816,63 @@ int hqs_graph_cancel(hqs_ctx* ctx, uint32_t n, const uint32_t* task, const uint3
         CU(cudaMemcpyAsync(ctx->g_new_ready.data(), ctx->d_gready, (size_t)k * 4, cudaMemcpyDeviceToHost, ctx->stream));
         CU(cudaStreamSynchronize(ctx->stream));
     }
-    if (cancelled) *cancelled = ctx->g_new_ready.data();
-    if (n_cancelled) *n_cancelled = k;
+    const u32* first = ctx->g_new_ready.data();
+    const u32* last = first + k;
+    if (ctx->shard_graph) {          // ascending: the owned handles are one run
+        first = std::lower_bound(first, last, ctx->g_lo);
+        last = std::lower_bound(first, last, ctx->g_hi);
+    }
+    if (cancelled) *cancelled = first;
+    if (n_cancelled) *n_cancelled = (u32)(last - first);
     return HQS_OK;
+}
+}  // namespace
+
+extern "C" {
+
+int hqs_graph_push(hqs_ctx* ctx, uint32_t n, const uint32_t* task, const uint32_t* class_id, const uint64_t* priority,
+                   const uint32_t* dep_off, const uint32_t* deps, uint32_t* n_ready) {
+    if (!ctx) return HQS_E_INVALID;
+    if (n_ready) *n_ready = 0;
+    if (int rc = graph_mode_check(ctx, "hqs_graph_push")) return rc;
+    return graph_push_impl(ctx, n, task, class_id, priority, dep_off, deps, n_ready);
+}
+
+int hqs_graph_finished(hqs_ctx* ctx, uint32_t n, const uint32_t* task, const uint32_t** new_ready, uint32_t* n_new_ready) {
+    if (!ctx) return HQS_E_INVALID;
+    ctx->g_new_ready.clear();
+    if (new_ready) *new_ready = ctx->g_new_ready.data();
+    if (n_new_ready) *n_new_ready = 0;
+    if (int rc = graph_mode_check(ctx, "hqs_graph_finished")) return rc;
+    return graph_finished_impl(ctx, n, task, new_ready, n_new_ready);
+}
+
+int hqs_graph_cancel(hqs_ctx* ctx, uint32_t n, const uint32_t* task, const uint32_t** cancelled, uint32_t* n_cancelled) {
+    if (!ctx) return HQS_E_INVALID;
+    ctx->g_new_ready.clear();
+    if (cancelled) *cancelled = ctx->g_new_ready.data();
+    if (n_cancelled) *n_cancelled = 0;
+    if (int rc = graph_mode_check(ctx, "hqs_graph_cancel")) return rc;
+    return graph_cancel_impl(ctx, n, task, cancelled, n_cancelled);
 }
 
 int hqs_graph_debug(hqs_ctx* ctx, uint64_t out[4]) {
     if (!ctx || !out) return HQS_E_INVALID;
-    if (int rc = graph_mode_check(ctx, "hqs_graph_debug")) return rc;
+    if (int rc = ctx->shard_graph ? shard_graph_mode_check(ctx, "hqs_graph_debug") : graph_mode_check(ctx, "hqs_graph_debug"))
+        return rc;
     CU(cudaSetDevice(ctx->device));
     unsigned long long* d_out = nullptr;
     CU(cudaMalloc(&d_out, 2 * sizeof(unsigned long long)));
     unsigned long long h[2] = {0, 0};
     cudaError_t e = cudaMemsetAsync(d_out, 0, sizeof h, ctx->stream);
-    if (e == cudaSuccess && ctx->n_handles) {
+    if (e == cudaSuccess && ctx->shard_graph) {
+        // the replicated lists over the global handles, the waiting tasks over the own keys
+        graph_debug_k<<<(ctx->g_total + 255) / 256, 256, 0, ctx->stream>>>(ctx->g_total, nullptr, ctx->d_ghead, ctx->d_pool, d_out);
+        if (ctx->n_handles)
+            graph_debug_k<<<(ctx->n_handles + 255) / 256, 256, 0, ctx->stream>>>(ctx->n_handles, ctx->d_key, nullptr, nullptr, d_out);
+        ctx->stats.kernel_launches += ctx->n_handles ? 2 : 1;
+        e = cudaGetLastError();
+    } else if (e == cudaSuccess && ctx->n_handles) {
         graph_debug_k<<<(ctx->n_handles + 255) / 256, 256, 0, ctx->stream>>>(ctx->n_handles, ctx->d_key,
                                                                            ctx->graph_storage ? ctx->d_ghead : nullptr, ctx->d_pool, d_out);
         ctx->stats.kernel_launches++;
@@ -1714,6 +1887,69 @@ int hqs_graph_debug(hqs_ctx* ctx, uint64_t out[4]) {
     out[2] = ctx->pool_compactions;
     out[3] = h[1];
     return HQS_OK;
+}
+
+int hqs_shard_graph_init(hqs_ctx* ctx, uint32_t n_total, uint32_t lo, uint32_t hi) {
+    if (!ctx) return HQS_E_INVALID;
+    if (ctx->shard_graph) return fail(ctx, HQS_E_STATE, "hqs_shard_graph_init was called before");
+    if (ctx->dag) return fail(ctx, HQS_E_STATE, "hqs_shard_graph_init is not available after hqs_dag_load");
+    if (ctx->graph) return fail(ctx, HQS_E_STATE, "hqs_shard_graph_init is not available after hqs_graph_push");
+    if (ctx->tick_pending) return fail(ctx, HQS_E_STATE, "the previous tick has not been fetched");
+    if (lo > hi || hi > n_total) return fail(ctx, HQS_E_INVALID, "owned range [%u, %u) is not inside [0, %u)", lo, hi, n_total);
+    if (n_total > GRAPH_NIL - 1024u) return fail(ctx, HQS_E_LIMIT, "n_total %u is too large", n_total);
+    CU(cudaSetDevice(ctx->device));
+    if (ctx->n_handles) {            // the replica must see every live task: the table must hold none yet
+        std::vector<u32> keys(ctx->n_handles);
+        CU(cudaMemcpyAsync(keys.data(), ctx->d_key, (size_t)ctx->n_handles * 4, cudaMemcpyDeviceToHost, ctx->stream));
+        CU(cudaStreamSynchronize(ctx->stream));
+        for (u32 k : keys)
+            if (k & KEY_VALID) return fail(ctx, HQS_E_STATE, "the task table already holds a live task");
+    }
+    const u32 cap = (n_total + 1023u) & ~1023u;
+    u32* gvalid = nullptr;
+    CU(cudaMalloc(&gvalid, (size_t)cap / 8));
+    CU(cudaMemsetAsync(gvalid, 0, (size_t)cap / 8, ctx->stream));
+    ctx->d_gvalid = gvalid;
+    ctx->shard_graph = true;
+    ctx->g_total = n_total;
+    ctx->g_lo = lo;
+    ctx->g_hi = hi;
+    ctx->graph_storage = false;      // arrays a graph call on the empty table may have made are re-made at the global size
+    int rc = ensure_graph_storage(ctx);
+    if (!rc) CU(cudaStreamSynchronize(ctx->stream));
+    return rc;
+}
+
+int hqs_shard_graph_push(hqs_ctx* ctx, uint32_t n, const uint32_t* task, const uint32_t* class_id, const uint64_t* priority,
+                         const uint32_t* dep_off, const uint32_t* deps, uint32_t* n_ready) {
+    if (!ctx) return HQS_E_INVALID;
+    if (n_ready) *n_ready = 0;
+    if (int rc = shard_graph_mode_check(ctx, "hqs_shard_graph_push")) return rc;
+    return shard_graph_outcome(ctx, graph_push_impl(ctx, n, task, class_id, priority, dep_off, deps, n_ready));
+}
+
+int hqs_shard_graph_finished(hqs_ctx* ctx, uint32_t n, const uint32_t* task, const uint32_t** new_ready, uint32_t* n_new_ready) {
+    if (!ctx) return HQS_E_INVALID;
+    ctx->g_new_ready.clear();
+    if (new_ready) *new_ready = ctx->g_new_ready.data();
+    if (n_new_ready) *n_new_ready = 0;
+    if (int rc = shard_graph_mode_check(ctx, "hqs_shard_graph_finished")) return rc;
+    return shard_graph_outcome(ctx, graph_finished_impl(ctx, n, task, new_ready, n_new_ready));
+}
+
+int hqs_shard_graph_cancel(hqs_ctx* ctx, uint32_t n, const uint32_t* task, const uint32_t** cancelled, uint32_t* n_cancelled) {
+    if (!ctx) return HQS_E_INVALID;
+    ctx->g_new_ready.clear();
+    if (cancelled) *cancelled = ctx->g_new_ready.data();
+    if (n_cancelled) *n_cancelled = 0;
+    if (int rc = shard_graph_mode_check(ctx, "hqs_shard_graph_cancel")) return rc;
+    return shard_graph_outcome(ctx, graph_cancel_impl(ctx, n, task, cancelled, n_cancelled));
+}
+
+int hqs_shard_graph_remove(hqs_ctx* ctx, uint32_t n, const uint32_t* task) {
+    if (!ctx) return HQS_E_INVALID;
+    if (int rc = shard_graph_mode_check(ctx, "hqs_shard_graph_remove")) return rc;
+    return shard_graph_outcome(ctx, shard_graph_remove_impl(ctx, n, task));
 }
 
 int hqs_tick_launch(hqs_ctx* ctx, uint32_t n_workers, const hqs_worker* workers, const uint64_t* free_rw,

@@ -203,6 +203,34 @@ def return_resources(s, h: np.ndarray) -> None:
     s._task_worker[h] = -1
 
 
+def cancel_bookkeeping(s, h: np.ndarray, gone: np.ndarray) -> Dict[int, List[int]]:
+    """The host's bookkeeping of on_cancel_tasks on the scheduler `s` whose handles `h` (named) and `gone` (what left the
+    table) are: a named task that is assigned gives its resources back, a prefilled one is no longer held, a retracting one
+    loses its redirect and the resources taken on the redirect target come back.  Returns worker id -> the named tasks to
+    cancel there, in the order they were named (the CancelTasks messages)."""
+    if h.size:
+        s._grow_tasks(int(h.max()) + 1)
+    left = set(gone.tolist())
+    messages: Dict[int, List[int]] = {}
+    assigned = []
+    for t in dict.fromkeys(h.tolist()):
+        if t not in left:
+            continue                                     # "Task is not here"
+        if t in s._retracting_from:
+            messages.setdefault(s._retracting_from.pop(t), []).append(t)
+            s.redirects.pop(t, None)
+            assigned.append(t)                           # try_remove_redirection: the target's resources come back
+        elif s._task_worker[t] >= 0:
+            messages.setdefault(int(s.worker_ids[s._task_worker[t]]), []).append(t)
+            assigned.append(t)
+        elif s._pf_worker[t] >= 0:
+            messages.setdefault(int(s._pf_worker[t]), []).append(t)
+            s._pf_worker[t] = -1
+    if assigned:
+        return_resources(s, np.array(assigned, dtype=np.int64))
+    return messages
+
+
 def query_workers(worker_totals: np.ndarray, remaining_s: Optional[np.ndarray] = None,
                   min_utilization: Optional[np.ndarray] = None) -> Tuple[np.ndarray, np.ndarray]:
     """The fake-worker array of a what-if query (new_worker_query): worker ids 0..n-1, time limits in seconds (inf = none)
@@ -505,13 +533,19 @@ class GpuScheduler:
 
     def _start_prefilled(self, handle: int, variant: int) -> int:
         """Bookkeeping of on_task_running_prefilled without the free vectors; returns the worker's index."""
+        pos = self._prefilled_started(handle, variant)
+        self.remove_ready_tasks(np.array([handle], dtype=np.uint32))
+        return pos
+
+    def _prefilled_started(self, handle: int, variant: int) -> int:
+        """The host half of _start_prefilled: the task now runs on the worker it was prefilled on; returns the worker's
+        index.  A sharded graph context takes the task out of its table on every rank instead (hqs_shard_graph_remove)."""
         wid = int(self._pf_worker[handle])
         assert wid >= 0, "task is not prefilled"
         pos = int(np.searchsorted(self.worker_ids, wid))
         self._pf_worker[handle] = -1
         self._task_worker[handle] = pos
         self._task_variant[handle] = variant
-        self.remove_ready_tasks(np.array([handle], dtype=np.uint32))
         return pos
 
     def _take_resources(self, pos: int, rq_id: int, variant: int) -> None:
@@ -617,26 +651,7 @@ class GpuScheduler:
         k = C.c_uint32(0)
         self._check(self._lib.hqs_graph_cancel(self._ctx, h.size, L.ptr(h), C.byref(ptr), C.byref(k)))
         gone = np.ctypeslib.as_array(ptr, shape=(k.value,)).copy() if k.value else np.zeros(0, dtype=np.uint32)
-        self._grow_tasks(int(h.max()) + 1)
-        left = set(gone.tolist())
-        messages: Dict[int, List[int]] = {}
-        assigned = []
-        for t in dict.fromkeys(h.tolist()):
-            if t not in left:
-                continue                                     # "Task is not here"
-            if t in self._retracting_from:
-                messages.setdefault(self._retracting_from.pop(t), []).append(t)
-                self.redirects.pop(t, None)
-                assigned.append(t)                           # try_remove_redirection: the target's resources come back
-            elif self._task_worker[t] >= 0:
-                messages.setdefault(int(self.worker_ids[self._task_worker[t]]), []).append(t)
-                assigned.append(t)
-            elif self._pf_worker[t] >= 0:
-                messages.setdefault(int(self._pf_worker[t]), []).append(t)
-                self._pf_worker[t] = -1
-        if assigned:
-            return_resources(self, np.array(assigned, dtype=np.int64))
-        return gone, messages
+        return gone, cancel_bookkeeping(self, h, gone)
 
     def graph_debug(self) -> np.ndarray:
         """hqs_graph_debug: [live edges, edge-pool capacity, pool compactions, waiting tasks]."""

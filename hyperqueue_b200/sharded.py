@@ -30,6 +30,11 @@ returns the same answer, the one a single context holding all ranks' tasks gives
 Priority levels are declared on every rank (hqs_levels_add), so that every rank numbers them identically, and are pruned
 by all ranks together at the start of a tick or a query (ShardedScheduler.prune_levels): a level is dropped only when no
 task of any rank carries it.
+
+Task graphs (ShardedScheduler.graph_init, then submit_tasks / graph_tasks_finished / graph_cancel_tasks): the graph is
+replicated on every rank (hqs_shard_graph_init) and every rank makes every graph call with the same GLOBAL arguments, runs
+the same propagation, writes the keys it owns and returns the handles it owns.  No graph data moves between ranks; the only
+collective is the free-vector all-reduce that finishing and cancelling already need.
 """
 from __future__ import annotations
 
@@ -41,7 +46,7 @@ import torch
 import torch.distributed as dist
 
 from . import _lib as L
-from .scheduler import WorkerTaskMapping, apply_tick_records, query_workers, return_resources
+from .scheduler import WorkerTaskMapping, apply_tick_records, cancel_bookkeeping, query_workers, return_resources
 
 
 def shard_exchange(counts_local: torch.Tensor, rank: int, world: int,
@@ -138,7 +143,9 @@ class ShardedScheduler:
                  group: Optional[dist.ProcessGroup] = None, p2p: bool = False) -> None:
         self.s = sched
         self.rank, self.world, self.group = rank, world, group
+        self.n_total = int(n_total)
         self.lo, self.hi = block_range(n_total, rank, world)
+        self.graph = False                  # graph_init was called: tasks enter and leave through the graph calls
         self.device = device
         self._counts = torch.zeros(L.HQS_MAX_GROUPS, dtype=torch.int32, device=device)
         self.p2p = bool(p2p)
@@ -148,6 +155,10 @@ class ShardedScheduler:
             attach_peers(sched, rank, world, group)
 
     def add_ready_tasks(self, handles, rq_ids, priorities) -> None:
+        if self.graph:                      # the replicated graph must see every live task
+            n = np.asarray(handles).size
+            self.submit_tasks(handles, rq_ids, priorities, np.zeros(n + 1, dtype=np.uint32), np.zeros(0, dtype=np.uint32))
+            return
         h = np.asarray(handles, dtype=np.int64)
         # every rank sees the whole call: number the priority levels identically everywhere
         lv = np.ascontiguousarray(np.unique(np.asarray(priorities, dtype=np.uint64)))
@@ -161,6 +172,11 @@ class ShardedScheduler:
         """TaskQueue::remove for GLOBAL handles, called with the same list on every rank: the owner of each task takes it
         out of its ready set.  Also the way to retire the handle of a finished task, so that it no longer keeps its
         priority level alive (prune_levels)."""
+        if self.graph:                      # every rank's replica forgets the handles too
+            h = np.ascontiguousarray(handles, dtype=np.uint32).reshape(-1)
+            if h.size:
+                self.s._check(self.s._lib.hqs_shard_graph_remove(self.s._ctx, h.size, L.ptr(h)))
+            return
         mine = self._mine(handles)
         if mine.size:
             self.s.remove_ready_tasks(mine.astype(np.uint32))
@@ -265,13 +281,15 @@ class ShardedScheduler:
     def on_task_running_prefilled(self, handle: int, variant: int) -> None:
         """The worker started one of its prefilled tasks (RunningPrefilled).  Only the owner knows the worker and the class,
         so the owner's (worker index, class) is summed over the ranks (one all-reduce of two integers), and every rank takes
-        the same resources from its replicated free vectors."""
+        the same resources from its replicated free vectors.  After graph_init the task leaves the table of every rank
+        (remove_ready_tasks: hqs_shard_graph_remove), so that no replica keeps it VALID."""
         s = self.s
         mine = self._mine([handle])
         key = np.zeros(2, dtype=np.int64)
         if mine.size:
             loc = int(mine[0])
-            key[:] = (s._start_prefilled(loc, variant) + 1, int(s._task_class[loc]) + 1)
+            pos = s._prefilled_started(loc, variant) if self.graph else s._start_prefilled(loc, variant)
+            key[:] = (pos + 1, int(s._task_class[loc]) + 1)
         if self.world > 1:
             t = torch.from_numpy(key)
             dev = self.device if dist.get_backend(self.group) == "nccl" else torch.device("cpu")
@@ -280,6 +298,8 @@ class ShardedScheduler:
             key = t.cpu().numpy()
         assert key[0] > 0, "task is not prefilled on any rank"
         s._take_resources(int(key[0]) - 1, int(key[1]) - 1, variant)
+        if self.graph:
+            self.remove_ready_tasks([handle])
 
     def on_retract_response(self, worker_id: int, handles) -> Dict[int, List[Tuple[int, int]]]:
         """The worker gave the listed tasks back; the owner of a redirected task returns it as target worker id ->
@@ -293,6 +313,93 @@ class ShardedScheduler:
         ret = self.s.dispose_prefill(rq_id)
         return {wid: [t + self.lo for t in lst] for wid, lst in ret.items()}
 
+    # task graphs: every rank is called with the same arguments; handles are GLOBAL --------------------------------------
+    def graph_init(self) -> None:
+        """Replicates the task graph over all n_total handles on this rank (hqs_shard_graph_init); call it on every rank
+        before any task is added.  From then on add_ready_tasks and remove_ready_tasks go through the graph calls."""
+        self.s._check(self.s._lib.hqs_shard_graph_init(self.s._ctx, self.n_total, self.lo, self.hi))
+        self.graph = True
+
+    def submit_tasks(self, handles, rq_ids, priorities, dep_off, deps) -> int:
+        """on_new_tasks with dependencies (GpuScheduler.submit_tasks) for GLOBAL handles: the batch's priorities are
+        declared first (hqs_levels_add), then every rank links the whole batch and pushes the keys it owns
+        (hqs_shard_graph_push).  Returns how many of this rank's tasks are ready at once."""
+        s = self.s
+        h = np.ascontiguousarray(handles, dtype=np.uint32).reshape(-1)
+        c = np.ascontiguousarray(rq_ids, dtype=np.uint32).reshape(-1)
+        p = np.ascontiguousarray(priorities, dtype=np.uint64).reshape(-1)
+        off = np.ascontiguousarray(dep_off, dtype=np.uint32)
+        d = np.ascontiguousarray(deps, dtype=np.uint32)
+        if not (h.shape == c.shape == p.shape) or off.shape != (h.size + 1,):
+            raise ValueError("shape mismatch")
+        if h.size == 0:
+            return 0
+        s._sync_classes()
+        lv = np.ascontiguousarray(np.unique(p))
+        s._check(s._lib.hqs_levels_add(s._ctx, lv.size, L.ptr(lv)))
+        n_ready = C.c_uint32(0)
+        s._check(s._lib.hqs_shard_graph_push(s._ctx, h.size, L.ptr(h), L.ptr(c), L.ptr(p), L.ptr(off),
+                                             L.ptr(d) if d.size else None, C.byref(n_ready)))
+        m = (h >= self.lo) & (h < self.hi)
+        if m.any():
+            loc = h[m] - np.uint32(self.lo)
+            s._grow_tasks(int(loc.max()) + 1)
+            s._task_class[loc] = c[m]
+            s._task_prio[loc] = p[m]
+        return int(n_ready.value)
+
+    def graph_tasks_finished(self, handles) -> np.ndarray:
+        """task_finished in a task graph (GpuScheduler.graph_tasks_finished) for GLOBAL handles: the owners return the
+        resources of their assigned tasks and the ranks sum the change of the free vectors, as tasks_finished does; every rank
+        releases consumers across the whole graph (hqs_shard_graph_finished).  Returns the newly ready handles this rank owns,
+        global and ascending: the ranks' lists in rank order are the single-context list."""
+        s = self.s
+        h = np.ascontiguousarray(handles, dtype=np.uint32).reshape(-1)
+        if h.size == 0:
+            return np.zeros(0, dtype=np.uint32)
+        ptr = C.POINTER(C.c_uint32)()
+        k = C.c_uint32(0)
+        s._check(s._lib.hqs_shard_graph_finished(s._ctx, h.size, L.ptr(h), C.byref(ptr), C.byref(k)))
+        ready = np.ctypeslib.as_array(ptr, shape=(k.value,)).copy() if k.value else np.zeros(0, dtype=np.uint32)
+        mine = self._mine(h)
+        before = s.free.copy()
+        if mine.size:
+            s._grow_tasks(int(mine.max()) + 1)
+            assigned = np.unique(mine[s._task_worker[mine] >= 0])
+            if assigned.size:
+                return_resources(s, assigned)
+        self._sum_free_change(before)
+        return ready
+
+    def graph_cancel_tasks(self, handles) -> Tuple[np.ndarray, Dict[int, List[int]]]:
+        """on_cancel_tasks / task_failed over a task graph (GpuScheduler.graph_cancel_tasks) for GLOBAL handles: every rank
+        removes the whole closure from its replica (hqs_shard_graph_cancel) and does the bookkeeping of its own named tasks;
+        the ranks then sum the change of the free vectors.  Returns (the part of the closure this rank owns, global and
+        ascending; worker id -> this rank's named tasks to cancel there, global handles)."""
+        s = self.s
+        h = np.ascontiguousarray(handles, dtype=np.uint32).reshape(-1)
+        if h.size == 0:
+            return np.zeros(0, dtype=np.uint32), {}
+        ptr = C.POINTER(C.c_uint32)()
+        k = C.c_uint32(0)
+        s._check(s._lib.hqs_shard_graph_cancel(s._ctx, h.size, L.ptr(h), C.byref(ptr), C.byref(k)))
+        gone = np.ctypeslib.as_array(ptr, shape=(k.value,)).copy() if k.value else np.zeros(0, dtype=np.uint32)
+        before = s.free.copy()
+        msgs = cancel_bookkeeping(s, self._mine(h), gone.astype(np.int64) - self.lo)
+        self._sum_free_change(before)
+        return gone, {wid: [t + self.lo for t in lst] for wid, lst in msgs.items()}
+
+    def _sum_free_change(self, before: np.ndarray) -> None:
+        """Returning resources only adds to a free vector: the per-worker change (>= 0, below the worker's total) is summed
+        over the ranks (one all-reduce of a [W][R] matrix, or nothing with world == 1)."""
+        s = self.s
+        if self.world > 1:
+            delta = (s.free - before).view(np.int64)
+            dev = self.device if dist.get_backend(self.group) == "nccl" else torch.device("cpu")
+            t = torch.from_numpy(np.ascontiguousarray(delta)).to(dev)
+            dist.all_reduce(t, group=self.group)
+            s.free = before + t.cpu().numpy().view(np.uint64)
+
     def tasks_finished(self, handles) -> None:
         """task_finished for GLOBAL handles, called with the same list on every rank: every rank holds the replicated free
         vectors, but only the owner of a task knows where it ran.  The owner returns the resources as GpuScheduler does
@@ -304,10 +411,4 @@ class ShardedScheduler:
         if mine.size:
             assert (s._task_worker[mine] >= 0).all(), "a finished task of this rank was never assigned"
             return_resources(s, mine)
-        if self.world > 1:
-            # finishing only adds to a free vector: the change is >= 0 and below the worker's total
-            delta = (s.free - before).view(np.int64)
-            dev = self.device if dist.get_backend(self.group) == "nccl" else torch.device("cpu")
-            t = torch.from_numpy(np.ascontiguousarray(delta)).to(dev)
-            dist.all_reduce(t, group=self.group)
-            s.free = before + t.cpu().numpy().view(np.uint64)
+        self._sum_free_change(before)

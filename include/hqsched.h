@@ -216,8 +216,8 @@ int hqs_tasks_finished(hqs_ctx* ctx, uint32_t n, const uint32_t* task, uint32_t*
  * cooperative kernel marks the whole closure); a marking that makes no progress for about a second fails with
  * HQS_E_CUDA and changes nothing.
  * hqs_ready_push / _range / _remove / _rearm, prefill, ticks, queries and the grouped fetch work unchanged on a graph
- * context.  HQS_E_STATE: the graph calls after hqs_dag_load, on a context attached with hqs_shard_attach, or while a tick or
- * query is pending; hqs_dag_load after a graph push.
+ * context.  HQS_E_STATE: the graph calls after hqs_dag_load, on a context attached with hqs_shard_attach or set up with
+ * hqs_shard_graph_init, or while a tick or query is pending; hqs_dag_load after a graph push.
  * hqs_graph_debug (debug / test aid, like hqs_debug_keys): out[0] live edges (linked into a producer's consumer list),
  * out[1] edge-pool capacity, out[2] pool compactions so far, out[3] waiting tasks (VALID, not READY, not DONE). */
 int hqs_graph_push(hqs_ctx* ctx, uint32_t n, const uint32_t* task, const uint32_t* class_id, const uint64_t* priority,
@@ -225,6 +225,40 @@ int hqs_graph_push(hqs_ctx* ctx, uint32_t n, const uint32_t* task, const uint32_
 int hqs_graph_finished(hqs_ctx* ctx, uint32_t n, const uint32_t* task, const uint32_t** new_ready, uint32_t* n_new_ready);
 int hqs_graph_cancel(hqs_ctx* ctx, uint32_t n, const uint32_t* task, const uint32_t** cancelled, uint32_t* n_cancelled);
 int hqs_graph_debug(hqs_ctx* ctx, uint64_t out[4]);
+
+/* Task graphs over a sharded ready set: the graph is replicated on every rank, each task's key lives on its owner.
+ * hqs_shard_graph_init: this context owns the GLOBAL handles [lo, hi) of a graph over n_total handles (its key table holds
+ * handle h at h - lo, as in the sharded tick) and allocates the replicated graph (the three per-handle arrays and the work
+ * list of hqs_graph_cancel, one VALID bit per handle, over all n_total handles, and the edge pool).  Allowed on attached
+ * contexts and on the contexts of the NCCL form.  HQS_E_STATE after hqs_dag_load or a hqs_graph_push, when the table holds a
+ * VALID key, a second time, or while a tick or query is pending; HQS_E_INVALID for lo > hi or hi > n_total.  From then on
+ * every task enters through hqs_shard_graph_push (a task without dependencies too), every remove goes through
+ * hqs_shard_graph_remove: hqs_ready_push, hqs_ready_push_range, hqs_ready_remove and the single-context graph calls return
+ * HQS_E_STATE, and the calls below return it on any other context.
+ * Every rank makes every call below with the same arguments (GLOBAL handles) and runs the same propagation on the same
+ * replicated state; no data moves between ranks.  A rank writes only the keys it owns and reports only the handles it owns,
+ * so the concatenation of the ranks' outputs in rank order is what one context holding every task returns.
+ * hqs_shard_graph_push: hqs_graph_push for the whole batch, with its contract and rejections; the bound for handles and
+ * dependencies is n_total (a handle or a dependency >= n_total rejects the batch on every rank).  Every priority of the batch
+ * must have been declared with hqs_levels_add (on every rank), and a class id >= n_classes is found on the host, so every rank
+ * rejects the same batches.  *n_ready counts this rank's tasks that are ready at once.
+ * hqs_shard_graph_finished: hqs_graph_finished; *new_ready = the newly ready handles this rank owns, global, ascending.
+ * hqs_shard_graph_cancel: hqs_graph_cancel; every rank marks the whole closure and removes it from its replica, and
+ * *cancelled = the part of the closure this rank owns, global, ascending.  The same six launches at any depth.
+ * hqs_shard_graph_remove: hqs_ready_remove for global handles: the owner's keys leave the table, every rank empties the
+ * handles' consumer lists and clears their graph VALID bits.  A handle >= n_total rejects the batch (HQS_E_INVALID).
+ * hqs_graph_debug answers on a sharded graph context: out[0..2] describe the replicated graph (equal on every rank), out[3]
+ * counts this rank's own waiting tasks.
+ * Every rejection (HQS_E_INVALID, HQS_E_STATE, HQS_E_LIMIT) follows from the arguments and the replicated state, so every rank
+ * rejects alike and nothing changes.  HQS_E_CUDA from any of these calls (a CUDA error, a failed allocation, the cancel
+ * marking's time-out) happens on one rank only and may leave that rank's replica different from the others: the context
+ * then refuses every sharded graph call with HQS_E_STATE, and the server must tear the sharded graph down on every rank. */
+int hqs_shard_graph_init(hqs_ctx* ctx, uint32_t n_total, uint32_t lo, uint32_t hi);
+int hqs_shard_graph_push(hqs_ctx* ctx, uint32_t n, const uint32_t* task, const uint32_t* class_id, const uint64_t* priority,
+                         const uint32_t* dep_off, const uint32_t* deps, uint32_t* n_ready);
+int hqs_shard_graph_finished(hqs_ctx* ctx, uint32_t n, const uint32_t* task, const uint32_t** new_ready, uint32_t* n_new_ready);
+int hqs_shard_graph_cancel(hqs_ctx* ctx, uint32_t n, const uint32_t* task, const uint32_t** cancelled, uint32_t* n_cancelled);
+int hqs_shard_graph_remove(hqs_ctx* ctx, uint32_t n, const uint32_t* task);
 
 /* One scheduler tick over the current ready set (replaces run_scheduling_solver + the task-selection
  * half of create_task_mapping).
