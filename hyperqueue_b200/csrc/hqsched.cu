@@ -66,6 +66,66 @@ typedef uint64_t u64;
 // ================================================================================================
 thread_local std::string g_create_error;
 
+// One owned allocation of n elements of T: device memory (Mem::Dev), page-locked host memory (Mem::Host), or page-locked
+// host memory mapped into the device's address space (Mem::Mapped, whose device alias is dev()).  Move-only: what it holds
+// is freed when it is destroyed or assigned over.  It converts to T*, so kernel launches take it as a raw pointer.
+enum class Mem { Dev, Host, Mapped };
+
+template <typename T, Mem M = Mem::Dev>
+class Buf {
+    T* p_ = nullptr;
+    T* dev_ = nullptr;
+    size_t n_ = 0;
+
+public:
+    Buf() = default;
+    Buf(Buf&& o) noexcept { swap(o); }
+    Buf& operator=(Buf&& o) noexcept { Buf(std::move(o)).swap(*this); return *this; }
+    ~Buf() {
+        if (p_ && M == Mem::Dev) cudaFree(p_);
+        else if (p_) cudaFreeHost(p_);
+    }
+    void swap(Buf& o) noexcept { std::swap(p_, o.p_); std::swap(dev_, o.dev_); std::swap(n_, o.n_); }
+    operator T*() const { return p_; }
+    T* dev() const { return dev_; }
+    size_t size() const { return n_; }
+
+    // Replaces the allocation by one of n elements.  keep: the current elements are copied to its front; fill >= 0: the
+    // elements not copied are set to that byte.  The old allocation is freed after `stream` has drained.  On failure the
+    // buffer is left as it was.
+    cudaError_t grow(size_t n, cudaStream_t stream, bool keep = false, int fill = -1) {
+        void* raw = nullptr;
+        cudaError_t e = M == Mem::Dev ? cudaMalloc(&raw, n * sizeof(T))
+                                      : cudaHostAlloc(&raw, n * sizeof(T), M == Mem::Mapped ? cudaHostAllocMapped : cudaHostAllocDefault);
+        if (e != cudaSuccess) return e;
+        Buf q;
+        q.p_ = static_cast<T*>(raw);
+        q.n_ = n;
+        const size_t kept = keep ? std::min(n_, n) : 0;
+        if (M == Mem::Mapped) e = cudaHostGetDevicePointer(reinterpret_cast<void**>(&q.dev_), raw, 0);
+        if (e == cudaSuccess && fill >= 0 && kept < n) {
+            if (M == Mem::Dev) e = cudaMemsetAsync(q.p_ + kept, fill, (n - kept) * sizeof(T), stream);
+            else memset(q.p_ + kept, fill, (n - kept) * sizeof(T));
+        }
+        if (e == cudaSuccess && kept) e = cudaMemcpyAsync(q.p_, p_, kept * sizeof(T), cudaMemcpyDefault, stream);
+        if (e == cudaSuccess && p_) e = cudaStreamSynchronize(stream);
+        if (e == cudaSuccess) swap(q);
+        return e;
+    }
+};
+
+// the tick's fixed-size buffers, set up together by the first call that sizes a tick (ensure_tick_buffers)
+struct TickBuffers {
+    Buf<u32> seg_cum, seg_wv;                 // [SEG_CAP] count segments
+    Buf<TickHeaderOut> hdr;
+    Buf<u64> free_after;
+    Buf<TickSync> sync;
+    Buf<u64> pk_fr; Buf<u32> pk_quota, pk_taken, pk_cand, pk_meta;
+    Buf<u32> rem_scratch; Buf<uint8_t> excl;
+    Buf<u32> pf_cum, pf_wk;                   // [PF_SEG_CAP] prefill segments
+    Buf<unsigned char, Mem::Mapped> h_hdr;    // TickHeaderOut + free_after, written by the kernel
+};
+
 }  // namespace
 
 struct hqs_ctx {
@@ -76,21 +136,19 @@ struct hqs_ctx {
     // classes
     u32 Q = 0;
     std::vector<hqs_class> classes;
-    unsigned char* d_classes = nullptr;   // ClassT<RT, u64>[Q]
-    u32 d_classes_cap = 0;                // bytes
-    unsigned char* d_classes32 = nullptr; // ClassT<RT, u32>[Q]: amounts / gscale[r] (valid when narrow_classes)
-    u32 d_classes32_cap = 0;
+    Buf<unsigned char> d_classes;         // ClassT<RT, u64>[Q]
+    Buf<unsigned char> d_classes32;       // ClassT<RT, u32>[Q]: amounts / gscale[r] (valid when narrow_classes)
     u32 class_bytes32 = 0;                // sizeof(ClassT<RT, u32>)
     u64 gscale[HQS_MAX_RESOURCES] = {};   // per-resource gcd of every requested amount (1 where nothing is requested)
     u64 narrow_limit[HQS_MAX_RESOURCES] = {};   // largest worker amount the narrow path can hold: gscale * (2^31 - 1)
     bool narrow_classes = false;          // every scaled class amount < 2^31
     // peer-to-peer sharded tick
-    u32* d_xbuf = nullptr;                // my exchange buffer: [2][HQS_MAX_PEERS][HQS_MAX_GROUPS] counts + [2][HQS_MAX_PEERS] flags
+    Buf<u32> d_xbuf;                      // my exchange buffer: [2][HQS_MAX_PEERS][HQS_MAX_GROUPS] counts + [2][HQS_MAX_PEERS] flags
     u32* x_peer[HQS_MAX_PEERS] = {};      // every rank's exchange buffer (own included), set by hqs_shard_attach
     std::vector<void*> x_opened;          // IPC mappings to close
     u32 x_world = 0, x_rank = 0, x_seq = 0;
-    u32* d_xall = nullptr;                // [HQS_MAX_GROUPS] sum over ranks, written by the solver
-    u32* d_xbefore = nullptr;             // [HQS_MAX_GROUPS] sum over lower ranks
+    Buf<u32> d_xall;                      // [HQS_MAX_GROUPS] sum over ranks, written by the solver
+    Buf<u32> d_xbefore;                   // [HQS_MAX_GROUPS] sum over lower ranks
     bool x_tick = false;                  // the tick being launched uses the exchange
     bool tick_narrow = false;             // this tick runs the narrow solver
     bool force_wide = false;              // hqs_create flag bit 1: always the 64-bit solver (tests)
@@ -102,81 +160,67 @@ struct hqs_ctx {
     bool coarse = false;
     bool levels_declared = false;   // hqs_levels_add was used: the caller numbers the levels (sharded ready set), no pruning
     size_t levels_pruned_at = 0;    // size of the level set after the last pruning
-    u64* d_levels = nullptr;
-    u32 d_levels_cap = 0;
-    u64* d_prune_lv = nullptr;      // prune_levels scratch: the exact levels and their live flags
-    u32* d_prune_live = nullptr;
-    u32 prune_cap = 0;
+    Buf<u64> d_levels;
+    Buf<u64> d_prune_lv;            // prune_levels scratch: the exact levels and their live flags
+    Buf<u32> d_prune_live;
     // task table
     u32 n_handles = 0, cap_handles = 0;
-    u32* d_key = nullptr;
-    u64* d_prio = nullptr;
-    u32* d_deps = nullptr;
-    u32* d_cons_off = nullptr;
-    u32* d_cons = nullptr;
+    Buf<u32> d_key;
+    Buf<u64> d_prio;
+    Buf<u32> d_deps, d_cons_off, d_cons;
     bool dag = false;
     // task graph (hqs_graph_push / hqs_graph_finished, hqs_graph.cuh): nothing of it exists before the first graph call
     bool graph_storage = false;         // the per-handle arrays below exist and grow with the table
     bool graph = false;                 // a graph push was accepted: hqs_dag_load is refused
-    u32* d_gdeps = nullptr; u32* d_ggen = nullptr; u32* d_ghead = nullptr;
-    u32* d_gbits = nullptr;             // [cap_handles / 32] ready bitmap of hqs_graph_finished (zero between calls)
-    u32* d_gready = nullptr;            // [cap_handles] the newly ready handles, ascending
-    u32* d_gblk = nullptr;              // [cap_handles / GRAPH_PER_BLOCK + 1] per-block sums of the ordered compactions
-    u32* d_gsmall = nullptr;            // [4] n_ready of a push, n_new of a finish, live edges of a compaction
-    GraphEdge* d_pool = nullptr;
+    Buf<u32> d_gdeps, d_ggen, d_ghead;
+    Buf<u32> d_gbits;                   // [cap_handles / 32] ready bitmap of hqs_graph_finished (zero between calls)
+    Buf<u32> d_gready;                  // [cap_handles] the newly ready handles, ascending
+    Buf<u32> d_gblk;                    // [cap_handles / GRAPH_PER_BLOCK + 1] per-block sums of the ordered compactions
+    Buf<u32> d_gsmall;                  // [4] n_ready of a push, n_new of a finish, live edges of a compaction
+    Buf<GraphEdge> d_pool;
     u32 pool_cap = 0, pool_used = 0;    // edge slots; slots [0, pool_used) have been handed out since the last compaction
     u64 pool_compactions = 0;
-    u32* d_gstage = nullptr; size_t gstage_cap = 0;   // a push's dependency offsets [n + 1] and dependencies
+    Buf<u32> d_gstage;                  // a push's dependency offsets [n + 1] and dependencies
     std::vector<u32> g_off, g_dep;      // host scratch of hqs_graph_push
     std::vector<std::pair<u32, u32>> g_pos;
     std::vector<u32> g_new_ready;       // what *new_ready of hqs_graph_finished / *cancelled of hqs_graph_cancel points to
-    u32* d_gwork = nullptr;             // [cap_handles] work list of hqs_graph_cancel's marking (GRAPH_NIL between calls)
-    GraphCancelSync* d_gcsync = nullptr;
+    Buf<u32> d_gwork;                   // [cap_handles] work list of hqs_graph_cancel's marking (GRAPH_NIL between calls)
+    Buf<GraphCancelSync> d_gcsync;
     // sharded graph (hqs_shard_graph_init): the graph arrays above are replicated over the global handles [0, g_total) and
     // keep that size; the key table holds the owned handles [g_lo, g_hi) at h - g_lo
     bool shard_graph = false;
     bool shard_graph_failed = false;    // a sharded graph call failed on the device: this replica may differ from the others
     u32 g_total = 0, g_lo = 0, g_hi = 0;
-    u32* d_gvalid = nullptr;            // [g_total / 32] the graph's VALID bits
+    Buf<u32> d_gvalid;                  // [g_total / 32] the graph's VALID bits
     // push staging (device)
-    u32* d_push_task = nullptr; u32* d_push_cls = nullptr; u64* d_push_prio = nullptr;
-    u32 push_cap = 0;
-    u32* d_newcnt = nullptr; u64* d_newprio = nullptr;
+    Buf<u32> d_push_task, d_push_cls; Buf<u64> d_push_prio;
+    Buf<u32> d_newcnt; Buf<u64> d_newprio;
     // tick buffers
     u32 sm_count = 132;
     u32 grid_ctas = 132;                // CTAs of the cooperative tick kernel (solver CTA + worker CTAs)
     u32 G_cap = 0, P_cap = 0;
-    u32* d_table = nullptr;
-    u32* d_total = nullptr;
-    GroupOut* d_gout = nullptr;
-    TickSync* d_sync = nullptr;
+    Buf<u32> d_table;
+    Buf<u32> d_total;
+    Buf<GroupOut> d_gout;
+    TickBuffers tick;
     size_t smem_budget[2] = {0, 0};     // dynamic shared memory a tick kernel instance may use (narrow, wide)
     bool sync_dirty = true;             // the counters must be zeroed before the next launch (first tick / after a failed one)
-    u64* d_pk_fr = nullptr; u32* d_pk_quota = nullptr; u32* d_pk_taken = nullptr; u32* d_pk_cand = nullptr; u32* d_pk_meta = nullptr;
-    u32* d_rem_scratch = nullptr; uint8_t* d_excl = nullptr;
     // proactive filling
     u32 pf_reserve = 0, pf_max = 0;     // SchedulerConfig::proactive_filling_reserve / _max (state.rs:14-21); max == 0: off
-    uint4* d_gout2 = nullptr; u32* d_pf_cum = nullptr; u32* d_pf_wk = nullptr;
+    Buf<uint4> d_gout2;
     std::vector<uint8_t> prefilled_wc; u32 prefilled_W = 0;   // host mirror for the next tick: [W][Q]
-    u32* d_seg_cum = nullptr; u32* d_seg_wv = nullptr;
-    hqs_assignment* d_out = nullptr; u32 out_cap_dev = 0;
-    TickHeaderOut* d_hdr = nullptr;
-    u64* d_free_after = nullptr;
-    unsigned char* d_tickin = nullptr; size_t tickin_cap = 0;   // device copy of the tick input (blocked mask; everything when zero-copy is off)
-    unsigned char* h_tickin = nullptr;  // pinned + mapped: the solver CTA reads the worker state from here
-    unsigned char* h_tickin_dev = nullptr;   // device-side address of h_tickin
+    Buf<hqs_assignment> d_out;
+    Buf<unsigned char> d_tickin;        // device copy of the tick input (blocked mask; everything when zero-copy is off)
+    Buf<unsigned char, Mem::Mapped> h_tickin;   // the solver CTA reads the worker state from here
     bool zero_copy = true;
-    unsigned char* h_hdr = nullptr;     // pinned + mapped: TickHeaderOut + free_after, written by the kernel
-    unsigned char* h_hdr_dev = nullptr;
-    size_t h_hdr_cap = 0;
-    u32* h_small = nullptr;             // pinned scratch (counters)
-    u32* h_pw = nullptr;                // pinned [HQS_MAX_WORKERS]: per-worker task counts of the last query
+    Buf<u32, Mem::Host> h_small;        // scratch (counters)
+    Buf<u32, Mem::Host> h_pw;           // [HQS_MAX_WORKERS]: per-worker task counts of the last query
     // per-worker grouping of the records (hqs_tick_fetch_grouped); nothing of it exists until the first grouped fetch or
     // hqs_grouped_reserve
-    hqs_assignment* d_grp_out = nullptr; u32 grp_cap = 0;      // the grouped records
-    u32* d_grp_hist = nullptr; size_t grp_hist_cap = 0;        // [2W + 1][tiles] counts, then their prefix over the tiles
-    u32* d_grp_small = nullptr;         // key totals [GRP_KEYS_MAX], offset table [GRP_KEYS_MAX + 1], the scan's ticket
-    u32* h_grp_off = nullptr;           // pinned mirror of the offset table
+    Buf<hqs_assignment> d_grp_out;      // the grouped records
+    Buf<u32> d_grp_hist;                // [2W + 1][tiles] counts, then their prefix over the tiles
+    Buf<u32> d_grp_small;               // key totals [GRP_KEYS_MAX], offset table [GRP_KEYS_MAX + 1], the scan's ticket
+    Buf<u32, Mem::Host> h_grp_off;      // mirror of the offset table
     float grp_ms = -1.f;                // device time of the last grouping (profiling on), < 0: none
     // last tick
     u32 last_W = 0, last_G = 0, last_L = 0;
@@ -191,6 +235,14 @@ struct hqs_ctx {
     float last_ms[4] = {0, 0, 0, 0};
     hqs_stats stats{};
     unsigned long long dbg[8] = {0};
+
+    // the buffers free themselves after this, once the stream has drained
+    ~hqs_ctx() {
+        if (stream) cudaStreamSynchronize(stream);
+        for (void* p : x_opened) cudaIpcCloseMemHandle(p);
+        for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e);
+        if (stream && own_stream) cudaStreamDestroy(stream);
+    }
 };
 
 namespace {
@@ -213,17 +265,18 @@ int fail(hqs_ctx* c, int code, const char* fmt, ...) {
                         __FILE__, __LINE__);                                                       \
     } while (0)
 
-template <typename T>
-int dev_realloc(hqs_ctx* ctx, T** p, size_t old_n, size_t new_n, bool keep, bool zero_new) {
-    T* q = nullptr;
-    CU(cudaMalloc(&q, new_n * sizeof(T)));
-    if (zero_new) CU(cudaMemsetAsync(q, 0, new_n * sizeof(T), ctx->stream));
-    if (keep && *p && old_n) CU(cudaMemcpyAsync(q, *p, old_n * sizeof(T), cudaMemcpyDeviceToDevice, ctx->stream));
-    if (*p) {
-        CU(cudaStreamSynchronize(ctx->stream));
-        CU(cudaFree(*p));
-    }
-    *p = q;
+// The per-handle graph arrays at cap handles, one after the other (their old and new sizes are never all held at once).
+// keep: the current entries stay; the new ones start with no dependencies, generation 0, an empty consumer list
+// (GRAPH_NIL) and no ready bit.  The cancel work list is GRAPH_NIL throughout.
+int size_graph_arrays(hqs_ctx* ctx, u32 cap, bool keep) {
+    cudaStream_t s = ctx->stream;
+    CU(ctx->d_gdeps.grow(cap, s, keep, 0));
+    CU(ctx->d_ggen.grow(cap, s, keep, 0));
+    CU(ctx->d_ghead.grow(cap, s, keep, 0xFF));
+    CU(ctx->d_gbits.grow(cap / 32, s, keep, 0));
+    CU(ctx->d_gready.grow(cap, s));
+    CU(ctx->d_gblk.grow(cap / GRAPH_PER_BLOCK + 1, s));
+    CU(ctx->d_gwork.grow(cap, s, false, 0xFF));
     return HQS_OK;
 }
 
@@ -231,20 +284,10 @@ int ensure_handles(hqs_ctx* ctx, u32 need) {
     if (need <= ctx->cap_handles) return HQS_OK;
     u32 cap = std::max<u32>(need, std::max<u32>(ctx->cap_handles * 2, 1u << 16));
     cap = (cap + 1023u) & ~1023u;
-    int rc;
-    if ((rc = dev_realloc(ctx, &ctx->d_key, ctx->cap_handles, cap, true, true))) return rc;
-    if ((rc = dev_realloc(ctx, &ctx->d_prio, ctx->cap_handles, cap, true, true))) return rc;
-    if (ctx->graph_storage && !ctx->shard_graph) {
-        if ((rc = dev_realloc(ctx, &ctx->d_gdeps, ctx->cap_handles, cap, true, true))) return rc;
-        if ((rc = dev_realloc(ctx, &ctx->d_ggen, ctx->cap_handles, cap, true, true))) return rc;
-        if ((rc = dev_realloc(ctx, &ctx->d_ghead, ctx->cap_handles, cap, true, false))) return rc;
-        CU(cudaMemsetAsync(ctx->d_ghead + ctx->cap_handles, 0xFF, (size_t)(cap - ctx->cap_handles) * 4, ctx->stream));
-        if ((rc = dev_realloc(ctx, &ctx->d_gbits, ctx->cap_handles / 32, cap / 32, true, true))) return rc;
-        if ((rc = dev_realloc(ctx, &ctx->d_gready, 0, cap, false, false))) return rc;
-        if ((rc = dev_realloc(ctx, &ctx->d_gblk, 0, cap / GRAPH_PER_BLOCK + 1, false, false))) return rc;
-        if ((rc = dev_realloc(ctx, &ctx->d_gwork, 0, cap, false, false))) return rc;
-        CU(cudaMemsetAsync(ctx->d_gwork, 0xFF, (size_t)cap * 4, ctx->stream));
-    }
+    CU(ctx->d_key.grow(cap, ctx->stream, true, 0));
+    CU(ctx->d_prio.grow(cap, ctx->stream, true, 0));
+    if (ctx->graph_storage && !ctx->shard_graph)
+        if (int rc = size_graph_arrays(ctx, cap, true)) return rc;
     ctx->cap_handles = cap;
     return HQS_OK;
 }
@@ -254,31 +297,19 @@ int ensure_handles(hqs_ctx* ctx, u32 need) {
 int ensure_graph_storage(hqs_ctx* ctx) {
     if (ctx->graph_storage) return HQS_OK;
     const u32 cap = ctx->shard_graph ? (ctx->g_total + 1023u) & ~1023u : ctx->cap_handles;
-    int rc;
-    if (!ctx->d_gsmall) CU(cudaMalloc(&ctx->d_gsmall, 4 * sizeof(u32)));
-    if (!ctx->d_gcsync) CU(cudaMalloc(&ctx->d_gcsync, sizeof(GraphCancelSync)));
-    if ((rc = dev_realloc(ctx, &ctx->d_gdeps, 0, cap, false, true))) return rc;
-    if ((rc = dev_realloc(ctx, &ctx->d_ggen, 0, cap, false, true))) return rc;
-    if ((rc = dev_realloc(ctx, &ctx->d_ghead, 0, cap, false, false))) return rc;
-    CU(cudaMemsetAsync(ctx->d_ghead, 0xFF, (size_t)cap * 4, ctx->stream));
-    if ((rc = dev_realloc(ctx, &ctx->d_gbits, 0, cap / 32, false, true))) return rc;
-    if ((rc = dev_realloc(ctx, &ctx->d_gready, 0, cap, false, false))) return rc;
-    if ((rc = dev_realloc(ctx, &ctx->d_gblk, 0, cap / GRAPH_PER_BLOCK + 1, false, false))) return rc;
-    if ((rc = dev_realloc(ctx, &ctx->d_gwork, 0, cap, false, false))) return rc;
-    CU(cudaMemsetAsync(ctx->d_gwork, 0xFF, (size_t)cap * 4, ctx->stream));
+    if (!ctx->d_gsmall) CU(ctx->d_gsmall.grow(4, ctx->stream));
+    if (!ctx->d_gcsync) CU(ctx->d_gcsync.grow(1, ctx->stream));
+    if (int rc = size_graph_arrays(ctx, cap, false)) return rc;
     ctx->graph_storage = true;
     return HQS_OK;
 }
 
 // device staging of a batch's handles (and class ids / priorities) for the ready-set calls
 int ensure_push_staging(hqs_ctx* ctx, u32 n) {
-    if (n <= ctx->push_cap) return HQS_OK;
-    CU(cudaStreamSynchronize(ctx->stream));
-    if (ctx->d_push_task) { CU(cudaFree(ctx->d_push_task)); CU(cudaFree(ctx->d_push_cls)); CU(cudaFree(ctx->d_push_prio)); }
-    ctx->push_cap = std::max<u32>(n, 1u << 16);
-    CU(cudaMalloc(&ctx->d_push_task, (size_t)ctx->push_cap * 4));
-    CU(cudaMalloc(&ctx->d_push_cls, (size_t)ctx->push_cap * 4));
-    CU(cudaMalloc(&ctx->d_push_prio, (size_t)ctx->push_cap * 8));
+    const u32 cap = std::max<u32>(n, 1u << 16);
+    if (n > ctx->d_push_task.size()) CU(ctx->d_push_task.grow(cap, ctx->stream));
+    if (n > ctx->d_push_cls.size()) CU(ctx->d_push_cls.grow(cap, ctx->stream));
+    if (n > ctx->d_push_prio.size()) CU(ctx->d_push_prio.grow(cap, ctx->stream));
     return HQS_OK;
 }
 
@@ -301,11 +332,7 @@ int upload_levels(hqs_ctx* ctx) {
         ctx->dev_levels.back() = 0;  // the last bucket takes everything below
     }
     const u32 n = (u32)ctx->dev_levels.size();
-    if (n > ctx->d_levels_cap) {
-        if (ctx->d_levels) { CU(cudaStreamSynchronize(ctx->stream)); CU(cudaFree(ctx->d_levels)); ctx->d_levels = nullptr; }
-        ctx->d_levels_cap = std::max<u32>(n * 2, 64);
-        CU(cudaMalloc(&ctx->d_levels, ctx->d_levels_cap * sizeof(u64)));
-    }
+    if (n > ctx->d_levels.size()) CU(ctx->d_levels.grow(std::max<u32>(n * 2, 64), ctx->stream));
     if (n) {
         // pageable source: the copy is staged by the runtime before the call returns
         CU(cudaMemcpyAsync(ctx->d_levels, ctx->dev_levels.data(), n * sizeof(u64), cudaMemcpyHostToDevice, ctx->stream));
@@ -330,16 +357,10 @@ int live_levels(hqs_ctx* ctx, std::vector<u32>& live) {
     const u32 L = (u32)ctx->levels.size();
     live.assign(L, 0);
     if (L == 0 || ctx->n_handles == 0) return HQS_OK;
-    // scratch kept across calls: a coarse table is pruned on every push that brings a new priority, and cudaFree would
+    // scratch kept across calls: a coarse table is pruned on every push that brings a new priority, and freeing would
     // synchronise the device each time
-    if (L > ctx->prune_cap) {
-        CU(cudaStreamSynchronize(ctx->stream));
-        if (ctx->d_prune_lv) { CU(cudaFree(ctx->d_prune_lv)); CU(cudaFree(ctx->d_prune_live)); }
-        ctx->d_prune_lv = nullptr; ctx->d_prune_live = nullptr;
-        ctx->prune_cap = std::max<u32>(L * 2, 4096);
-        CU(cudaMalloc(&ctx->d_prune_lv, (size_t)ctx->prune_cap * 8));
-        CU(cudaMalloc(&ctx->d_prune_live, (size_t)ctx->prune_cap * 4));
-    }
+    if (L > ctx->d_prune_lv.size()) CU(ctx->d_prune_lv.grow(std::max<u32>(L * 2, 4096), ctx->stream));
+    if (L > ctx->d_prune_live.size()) CU(ctx->d_prune_live.grow(std::max<u32>(L * 2, 4096), ctx->stream));
     u64* d_lv = ctx->d_prune_lv;
     u32* d_live = ctx->d_prune_live;
     CU(cudaMemsetAsync(d_live, 0, (size_t)L * 4, ctx->stream));
@@ -424,51 +445,39 @@ void distinct_priorities(const u64* p, u32 n, std::vector<u64>& out) {
 int ensure_tick_buffers(hqs_ctx* ctx, u32 G, u32 P, u32 W, u32 out_cap) {
     if (G > ctx->G_cap || P > ctx->P_cap || (size_t)G * P > (size_t)ctx->G_cap * ctx->P_cap) {
         const u32 ng = std::max(G, ctx->G_cap), np = std::max(P, ctx->P_cap);
-        CU(cudaStreamSynchronize(ctx->stream));
-        if (ctx->d_table) CU(cudaFree(ctx->d_table));
-        CU(cudaMalloc(&ctx->d_table, (size_t)ng * np * sizeof(u32)));
+        cudaStream_t s = ctx->stream;
+        CU(ctx->d_table.grow((size_t)ng * np, s));
         if (ng > ctx->G_cap) {
-            if (ctx->d_total) CU(cudaFree(ctx->d_total));
-            if (ctx->d_gout) CU(cudaFree(ctx->d_gout));
-            CU(cudaMalloc(&ctx->d_total, ng * sizeof(u32)));
-            CU(cudaMemsetAsync(ctx->d_total, 0, ng * sizeof(u32), ctx->stream));
-            CU(cudaMalloc(&ctx->d_gout, ng * sizeof(GroupOut)));
-            CU(cudaMemsetAsync(ctx->d_gout, 0, ng * sizeof(GroupOut), ctx->stream));
-            if (ctx->d_gout2) CU(cudaFree(ctx->d_gout2));
-            CU(cudaMalloc(&ctx->d_gout2, ng * sizeof(uint4)));
-            CU(cudaMemsetAsync(ctx->d_gout2, 0, ng * sizeof(uint4), ctx->stream));
+            CU(ctx->d_total.grow(ng, s, false, 0));
+            CU(ctx->d_gout.grow(ng, s, false, 0));
+            CU(ctx->d_gout2.grow(ng, s, false, 0));
         }
         ctx->G_cap = ng; ctx->P_cap = np;
     }
-    if (!ctx->d_seg_cum) {
-        CU(cudaMalloc(&ctx->d_seg_cum, SEG_CAP * sizeof(u32)));
-        CU(cudaMalloc(&ctx->d_seg_wv, SEG_CAP * sizeof(u32)));
-        CU(cudaMalloc(&ctx->d_hdr, sizeof(TickHeaderOut)));
-        CU(cudaMalloc(&ctx->d_free_after, (size_t)HQS_MAX_WORKERS * HQS_MAX_RESOURCES * sizeof(u64)));
-        CU(cudaMalloc(&ctx->d_sync, sizeof(TickSync)));
-        CU(cudaMalloc(&ctx->d_pk_fr, (size_t)HQS_MAX_WORKERS * HQS_MAX_RESOURCES * sizeof(u64)));
-        CU(cudaMalloc(&ctx->d_pk_quota, (size_t)HQS_MAX_WORKERS * PACK_MAX_CAND * sizeof(u32)));
-        CU(cudaMalloc(&ctx->d_pk_taken, (size_t)HQS_MAX_WORKERS * PACK_MAX_CAND * sizeof(u32)));
-        CU(cudaMalloc(&ctx->d_pk_cand, PACK_MAX_CAND * sizeof(u32)));
-        CU(cudaMalloc(&ctx->d_pk_meta, 2 * sizeof(u32)));
-        CU(cudaMalloc(&ctx->d_rem_scratch, (size_t)HQS_MAX_WORKERS * HQS_MAX_RESOURCES * sizeof(u64)));
-        CU(cudaMalloc(&ctx->d_excl, HQS_MAX_WORKERS));
-        CU(cudaMalloc(&ctx->d_pf_cum, PF_SEG_CAP * sizeof(u32)));
-        CU(cudaMalloc(&ctx->d_pf_wk, PF_SEG_CAP * sizeof(u32)));
+    if (!ctx->tick.hdr) {
+        const size_t wr = (size_t)HQS_MAX_WORKERS * HQS_MAX_RESOURCES;
+        const size_t wc = (size_t)HQS_MAX_WORKERS * PACK_MAX_CAND;
+        cudaStream_t s = ctx->stream;
+        TickBuffers b;
+        CU(b.seg_cum.grow(SEG_CAP, s));
+        CU(b.seg_wv.grow(SEG_CAP, s));
+        CU(b.hdr.grow(1, s));
+        CU(b.free_after.grow(wr, s));
+        CU(b.sync.grow(1, s));
+        CU(b.pk_fr.grow(wr, s));
+        CU(b.pk_quota.grow(wc, s));
+        CU(b.pk_taken.grow(wc, s));
+        CU(b.pk_cand.grow(PACK_MAX_CAND, s));
+        CU(b.pk_meta.grow(2, s));
+        CU(b.rem_scratch.grow(wr * sizeof(u64) / sizeof(u32), s));
+        CU(b.excl.grow(HQS_MAX_WORKERS, s));
+        CU(b.pf_cum.grow(PF_SEG_CAP, s));
+        CU(b.pf_wk.grow(PF_SEG_CAP, s));
+        CU(b.h_hdr.grow(sizeof(TickHeaderOut) + wr * 8, s, false, 0));
+        ctx->tick = std::move(b);
         ctx->sync_dirty = true;
     }
-    if (!ctx->h_hdr) {
-        ctx->h_hdr_cap = sizeof(TickHeaderOut) + (size_t)HQS_MAX_WORKERS * HQS_MAX_RESOURCES * 8;
-        CU(cudaHostAlloc(&ctx->h_hdr, ctx->h_hdr_cap, cudaHostAllocMapped));
-        memset(ctx->h_hdr, 0, ctx->h_hdr_cap);
-        CU(cudaHostGetDevicePointer(reinterpret_cast<void**>(&ctx->h_hdr_dev), ctx->h_hdr, 0));
-    }
-    if (out_cap > ctx->out_cap_dev) {
-        CU(cudaStreamSynchronize(ctx->stream));
-        if (ctx->d_out) CU(cudaFree(ctx->d_out));
-        ctx->out_cap_dev = std::max<u32>(out_cap, 1024);
-        CU(cudaMalloc(&ctx->d_out, (size_t)ctx->out_cap_dev * sizeof(hqs_assignment)));
-    }
+    if (out_cap > ctx->d_out.size()) CU(ctx->d_out.grow(std::max<u32>(out_cap, 1024), ctx->stream));
     (void)W;
     return HQS_OK;
 }
@@ -580,15 +589,8 @@ TickGeom tick_geom(const hqs_ctx* ctx) {
 }
 
 int ensure_tickin(hqs_ctx* ctx, size_t bytes) {
-    if (bytes <= ctx->tickin_cap) return HQS_OK;
-    CU(cudaStreamSynchronize(ctx->stream));
-    if (ctx->d_tickin) CU(cudaFree(ctx->d_tickin));
-    if (ctx->h_tickin) CU(cudaFreeHost(ctx->h_tickin));
-    ctx->d_tickin = nullptr; ctx->h_tickin = nullptr;
-    ctx->tickin_cap = bytes * 2;
-    CU(cudaMalloc(&ctx->d_tickin, ctx->tickin_cap));
-    CU(cudaHostAlloc(&ctx->h_tickin, ctx->tickin_cap, cudaHostAllocMapped));
-    CU(cudaHostGetDevicePointer(reinterpret_cast<void**>(&ctx->h_tickin_dev), ctx->h_tickin, 0));
+    if (bytes > ctx->d_tickin.size()) CU(ctx->d_tickin.grow(bytes * 2, ctx->stream));
+    if (bytes > ctx->h_tickin.size()) CU(ctx->h_tickin.grow(bytes * 2, ctx->stream));
     return HQS_OK;
 }
 
@@ -682,7 +684,7 @@ const void* tick_fn(u32 RT, bool narrow) {
 TickArgs base_args(hqs_ctx* ctx, const TickGeom& t, u32 W, const TickLayout& lay, bool blocked) {
     TickArgs a;
     memset(&a, 0, sizeof a);
-    const unsigned char* in = ctx->zero_copy ? ctx->h_tickin_dev : ctx->d_tickin;
+    const unsigned char* in = ctx->zero_copy ? ctx->h_tickin.dev() : ctx->d_tickin;
     a.free_rw = reinterpret_cast<const u64*>(in + lay.off_free);
     a.total_rw = reinterpret_cast<const u64*>(in + lay.off_total);
     a.rem_time = reinterpret_cast<const u64*>(in + lay.off_rem);
@@ -702,19 +704,20 @@ TickArgs base_args(hqs_ctx* ctx, const TickGeom& t, u32 W, const TickLayout& lay
     a.total_local = ctx->d_total;
     a.table = ctx->d_table;
     a.gout = ctx->d_gout;
-    a.seg_cum = ctx->d_seg_cum; a.seg_wv = ctx->d_seg_wv;
-    a.free_after = ctx->d_free_after;
-    a.hdr = ctx->d_hdr;
-    a.hdr_host = reinterpret_cast<TickHeaderOut*>(ctx->h_hdr_dev);
+    const TickBuffers& tb = ctx->tick;
+    a.seg_cum = tb.seg_cum; a.seg_wv = tb.seg_wv;
+    a.free_after = tb.free_after;
+    a.hdr = tb.hdr;
+    a.hdr_host = reinterpret_cast<TickHeaderOut*>(tb.h_hdr.dev());
     a.out = ctx->d_out;
-    a.rem_scratch = ctx->d_rem_scratch;
-    a.sync = ctx->d_sync;
-    a.pk.fr = ctx->d_pk_fr; a.pk.quota = ctx->d_pk_quota; a.pk.taken = ctx->d_pk_taken;
-    a.pk.cand = ctx->d_pk_cand; a.pk.meta = ctx->d_pk_meta;
-    a.excl_glob = ctx->d_excl;
+    a.rem_scratch = tb.rem_scratch;
+    a.sync = tb.sync;
+    a.pk.fr = tb.pk_fr; a.pk.quota = tb.pk_quota; a.pk.taken = tb.pk_taken;
+    a.pk.cand = tb.pk_cand; a.pk.meta = tb.pk_meta;
+    a.excl_glob = tb.excl;
     a.pf_shift = ctx->pf_max ? 1 : 0; a.pf_reserve = ctx->pf_reserve; a.pf_max = ctx->pf_max;
     a.prefilled_wc = ctx->h_small[11] ? ctx->d_tickin + lay.off_pfwc : nullptr;
-    a.gout2 = ctx->d_gout2; a.pf_cum = ctx->d_pf_cum; a.pf_wk = ctx->d_pf_wk;
+    a.gout2 = ctx->d_gout2; a.pf_cum = tb.pf_cum; a.pf_wk = tb.pf_wk;
     return a;
 }
 
@@ -775,7 +778,7 @@ int launch_tick(hqs_ctx* ctx, const TickGeom& t, u32 W, const TickLayout& lay, b
     const size_t smem = std::max(solver_smem, t.worker_smem);
     if (smem > budget) return fail(ctx, HQS_E_LIMIT, "tick needs %zu bytes of shared memory, %zu available", smem, budget);
     if (ctx->sync_dirty) {
-        CU(cudaMemsetAsync(ctx->d_sync, 0, sizeof(TickSync), ctx->stream));
+        CU(cudaMemsetAsync(ctx->tick.sync, 0, sizeof(TickSync), ctx->stream));
         ctx->sync_dirty = false;
     }
     ctx->ev_valid = false;
@@ -794,7 +797,7 @@ int launch_tick(hqs_ctx* ctx, const TickGeom& t, u32 W, const TickLayout& lay, b
 // waits for the tick kernel and reads the header the kernel wrote into the pinned mirror
 int wait_header(hqs_ctx* ctx, TickHeaderOut* hdr) {
     CU(cudaStreamSynchronize(ctx->stream));
-    memcpy(hdr, ctx->h_hdr, sizeof *hdr);
+    memcpy(hdr, ctx->tick.h_hdr, sizeof *hdr);
     ctx->stats.n_groups = hdr->n_groups;
     ctx->stats.n_levels = ctx->last_L;
     ctx->stats.n_assigned = hdr->n_assigned;
@@ -835,7 +838,7 @@ int ensure_query_buffers(hqs_ctx* ctx) {
     if (ctx->h_pw) return HQS_OK;
     cudaFuncAttributes fa;
     CU(cudaFuncGetAttributes(&fa, (const void*)seg_worker_totals_k));
-    CU(cudaMallocHost(&ctx->h_pw, HQS_MAX_WORKERS * sizeof(u32)));
+    CU(ctx->h_pw.grow(HQS_MAX_WORKERS, ctx->stream));
     return HQS_OK;
 }
 
@@ -848,9 +851,9 @@ int launch_query(hqs_ctx* ctx, const TickGeom& t, u32 W, const TickLayout& lay, 
     if (rc) return rc;
     rc = launch_tick(ctx, t, W, lay, blocked, d_counts_all, nullptr, 0, false, exchange);
     if (rc) return rc;
-    u32* d_pw = ctx->d_pk_quota;    // scratch (pack is over): [W] counters
+    u32* d_pw = ctx->tick.pk_quota;    // scratch (pack is over): [W] counters
     CU(cudaMemsetAsync(d_pw, 0, W * sizeof(u32), ctx->stream));
-    seg_worker_totals_k<<<(t.G + 127) / 128, 128, 0, ctx->stream>>>(ctx->d_gout, t.G, ctx->d_seg_cum, ctx->d_seg_wv, d_pw);
+    seg_worker_totals_k<<<(t.G + 127) / 128, 128, 0, ctx->stream>>>(ctx->d_gout, t.G, ctx->tick.seg_cum, ctx->tick.seg_wv, d_pw);
     ctx->stats.kernel_launches++;
     CU(cudaGetLastError());
     CU(cudaMemcpyAsync(ctx->h_pw, d_pw, W * sizeof(u32), cudaMemcpyDeviceToHost, ctx->stream));
@@ -889,25 +892,16 @@ int ensure_group_buffers(hqs_ctx* ctx, u32 W, u32 cap) {
         CU(cudaFuncGetAttributes(&fa, (const void*)group_scatter_k));
         CU(cudaFuncSetAttribute((const void*)group_scatter_k, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                 (int)group_scatter_smem(HQS_MAX_WORKERS)));
-        CU(cudaMallocHost(&ctx->h_grp_off, (GRP_KEYS_MAX + 1) * sizeof(u32)));
-        CU(cudaMalloc(&ctx->d_grp_small, (2 * GRP_KEYS_MAX + 2) * sizeof(u32)));
-        CU(cudaMemsetAsync(ctx->d_grp_small, 0, (2 * GRP_KEYS_MAX + 2) * sizeof(u32), ctx->stream));   // the ticket starts at 0
+        Buf<u32, Mem::Host> off;
+        Buf<u32> small;
+        CU(off.grow(GRP_KEYS_MAX + 1, ctx->stream));
+        CU(small.grow(2 * GRP_KEYS_MAX + 2, ctx->stream, false, 0));   // the ticket starts at 0
+        ctx->h_grp_off = std::move(off);
+        ctx->d_grp_small = std::move(small);
     }
-    if (cap > ctx->grp_cap) {
-        CU(cudaStreamSynchronize(ctx->stream));
-        if (ctx->d_grp_out) CU(cudaFree(ctx->d_grp_out));
-        ctx->d_grp_out = nullptr;
-        ctx->grp_cap = std::max<u32>(cap, 1024);
-        CU(cudaMalloc(&ctx->d_grp_out, (size_t)ctx->grp_cap * sizeof(hqs_assignment)));
-    }
-    const size_t need = (size_t)(2 * W + 1) * ((ctx->grp_cap + GROUP_TILE - 1) / GROUP_TILE);
-    if (need > ctx->grp_hist_cap) {
-        CU(cudaStreamSynchronize(ctx->stream));
-        if (ctx->d_grp_hist) CU(cudaFree(ctx->d_grp_hist));
-        ctx->d_grp_hist = nullptr;
-        ctx->grp_hist_cap = need;
-        CU(cudaMalloc(&ctx->d_grp_hist, need * sizeof(u32)));
-    }
+    if (cap > ctx->d_grp_out.size()) CU(ctx->d_grp_out.grow(std::max<u32>(cap, 1024), ctx->stream));
+    const size_t need = (2 * W + 1) * ((ctx->d_grp_out.size() + GROUP_TILE - 1) / GROUP_TILE);
+    if (need > ctx->d_grp_hist.size()) CU(ctx->d_grp_hist.grow(need, ctx->stream));
     return HQS_OK;
 }
 
@@ -943,7 +937,7 @@ int tick_fetch_impl(hqs_ctx* ctx, u32 out_cap, hqs_assignment* out, u32* out_n, 
     const u32 n_rec = hdr.n_assigned + hdr.n_prefilled;           // assignments (kind 0 / 2), then prefills (kind 1)
     if (hdr.error == 3 || n_rec > out_cap || (n_rec && !out))
         return fail(ctx, HQS_E_OVERFLOW, "out_cap=%u too small for %u assignments + %u prefills", out_cap, hdr.n_assigned, hdr.n_prefilled);
-    if (free_after) memcpy(free_after, ctx->h_hdr + sizeof(TickHeaderOut), (size_t)ctx->last_W * ctx->R * 8);
+    if (free_after) memcpy(free_after, ctx->tick.h_hdr + sizeof(TickHeaderOut), (size_t)ctx->last_W * ctx->R * 8);
     const u32 W = ctx->last_W, n_off = 2 * W + 2;
     if (worker_off) memset(worker_off, 0, n_off * sizeof(u32));
     if (n_rec && !worker_off) {
@@ -952,7 +946,7 @@ int tick_fetch_impl(hqs_ctx* ctx, u32 out_cap, hqs_assignment* out, u32* out_n, 
     } else if (n_rec) {
         // n and the error word are known here, so the grids are exact and a failed tick never reaches this point
         ctx->grp_ms = -1.f;
-        if ((rc = ensure_group_buffers(ctx, W, std::max(n_rec, ctx->out_cap_dev)))) return rc;
+        if ((rc = ensure_group_buffers(ctx, W, std::max(n_rec, (u32)ctx->d_out.size())))) return rc;
         if ((rc = launch_grouping(ctx, n_rec, W))) return rc;
         CU(cudaMemcpyAsync(out, ctx->d_grp_out, (size_t)n_rec * sizeof(hqs_assignment), cudaMemcpyDeviceToHost, ctx->stream));
         CU(cudaMemcpyAsync(ctx->h_grp_off, ctx->d_grp_small + GRP_KEYS_MAX, n_off * sizeof(u32), cudaMemcpyDeviceToHost, ctx->stream));
@@ -998,11 +992,12 @@ int hqs_create(hqs_ctx** out, int device, uint32_t n_resources, uint32_t flags) 
     ctx->force_wide = (flags & 2u) != 0;
     e = cudaSetDevice(device);
     if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking);
+    if (e != cudaSuccess) ctx->stream = nullptr;   // not a stream after a failed create: nothing to destroy
     int sms = 0;
     if (e == cudaSuccess) e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
-    if (e == cudaSuccess) e = cudaMalloc(&ctx->d_newcnt, 2 * sizeof(u32));
-    if (e == cudaSuccess) e = cudaMalloc(&ctx->d_newprio, NEWPRIO_CAP * sizeof(u64));
-    if (e == cudaSuccess) e = cudaMallocHost(&ctx->h_small, 64 * sizeof(u32));
+    if (e == cudaSuccess) e = ctx->d_newcnt.grow(2, ctx->stream);
+    if (e == cudaSuccess) e = ctx->d_newprio.grow(NEWPRIO_CAP, ctx->stream);
+    if (e == cudaSuccess) e = ctx->h_small.grow(64, ctx->stream);
     {
         const void* fns[] = {(const void*)tick_k<4, u32>, (const void*)tick_k<8, u32>, (const void*)tick_k<16, u32>,
                              (const void*)tick_k<4, u64>, (const void*)tick_k<8, u64>, (const void*)tick_k<16, u64>};
@@ -1042,29 +1037,6 @@ int hqs_create(hqs_ctx** out, int device, uint32_t n_resources, uint32_t flags) 
 void hqs_destroy(hqs_ctx* ctx) {
     if (!ctx) return;
     cudaSetDevice(ctx->device);
-    if (ctx->stream) cudaStreamSynchronize(ctx->stream);
-    void* dev_ptrs[] = {ctx->d_classes, ctx->d_classes32, ctx->d_levels, ctx->d_key, ctx->d_prio, ctx->d_deps, ctx->d_cons_off,
-                        ctx->d_cons, ctx->d_push_task, ctx->d_push_cls, ctx->d_push_prio, ctx->d_newcnt,
-                        ctx->d_newprio, ctx->d_table, ctx->d_total, ctx->d_gout, ctx->d_rem_scratch, ctx->d_excl, ctx->d_gout2, ctx->d_pf_cum, ctx->d_pf_wk, ctx->d_seg_cum,
-                        ctx->d_seg_wv, ctx->d_out, ctx->d_hdr, ctx->d_free_after, ctx->d_tickin, ctx->d_sync, ctx->d_pk_fr,
-                        ctx->d_pk_quota, ctx->d_pk_taken, ctx->d_pk_cand, ctx->d_pk_meta, ctx->d_prune_lv, ctx->d_prune_live,
-                        ctx->d_gdeps, ctx->d_ggen, ctx->d_ghead, ctx->d_gbits, ctx->d_gready, ctx->d_gblk, ctx->d_gsmall,
-                        ctx->d_pool, ctx->d_gstage, ctx->d_gwork, ctx->d_gcsync, ctx->d_gvalid};
-    for (void* p : dev_ptrs) if (p) cudaFree(p);
-    for (void* p : ctx->x_opened) cudaIpcCloseMemHandle(p);
-    if (ctx->d_xbuf) cudaFree(ctx->d_xbuf);
-    if (ctx->d_xall) cudaFree(ctx->d_xall);
-    if (ctx->d_xbefore) cudaFree(ctx->d_xbefore);
-    if (ctx->h_tickin) cudaFreeHost(ctx->h_tickin);
-    if (ctx->h_hdr) cudaFreeHost(ctx->h_hdr);
-    if (ctx->h_small) cudaFreeHost(ctx->h_small);
-    if (ctx->h_pw) cudaFreeHost(ctx->h_pw);
-    if (ctx->d_grp_out) cudaFree(ctx->d_grp_out);
-    if (ctx->d_grp_hist) cudaFree(ctx->d_grp_hist);
-    if (ctx->d_grp_small) cudaFree(ctx->d_grp_small);
-    if (ctx->h_grp_off) cudaFreeHost(ctx->h_grp_off);
-    for (cudaEvent_t e : ctx->ev) if (e) cudaEventDestroy(e);
-    if (ctx->stream && ctx->own_stream) cudaStreamDestroy(ctx->stream);
     delete ctx;
 }
 
@@ -1098,12 +1070,7 @@ int hqs_classes_set(hqs_ctx* ctx, uint32_t n_classes, const hqs_class* classes) 
         }
     }
     CU(cudaSetDevice(ctx->device));
-    if (blob.size() > ctx->d_classes_cap) {
-        CU(cudaStreamSynchronize(ctx->stream));
-        if (ctx->d_classes) CU(cudaFree(ctx->d_classes));
-        ctx->d_classes_cap = (u32)std::max<size_t>(blob.size() * 2, 4096);
-        CU(cudaMalloc(&ctx->d_classes, ctx->d_classes_cap));
-    }
+    if (blob.size() > ctx->d_classes.size()) CU(ctx->d_classes.grow(std::max<size_t>(blob.size() * 2, 4096), ctx->stream));
     CU(cudaMemcpyAsync(ctx->d_classes, blob.data(), blob.size(), cudaMemcpyHostToDevice, ctx->stream));
     // narrow copy: amounts divided by the per-resource gcd of everything requested
     u64 gs[HQS_MAX_RESOURCES];
@@ -1134,12 +1101,8 @@ int hqs_classes_set(hqs_ctx* ctx, uint32_t n_classes, const hqs_class* classes) 
         }
     }
     ctx->narrow_classes = narrow_ok;
-    if (blob32.size() > ctx->d_classes32_cap) {
-        CU(cudaStreamSynchronize(ctx->stream));
-        if (ctx->d_classes32) CU(cudaFree(ctx->d_classes32));
-        ctx->d_classes32_cap = (u32)std::max<size_t>(blob32.size() * 2, 4096);
-        CU(cudaMalloc(&ctx->d_classes32, ctx->d_classes32_cap));
-    }
+    if (blob32.size() > ctx->d_classes32.size())
+        CU(ctx->d_classes32.grow(std::max<size_t>(blob32.size() * 2, 4096), ctx->stream));
     CU(cudaMemcpyAsync(ctx->d_classes32, blob32.data(), blob32.size(), cudaMemcpyHostToDevice, ctx->stream));
     CU(cudaStreamSynchronize(ctx->stream));
     const bool q_changed = ctx->Q != n_classes;
@@ -1220,7 +1183,7 @@ int push_impl(hqs_ctx* ctx, u32 n, const u32* task, u32 first_handle, const u32*
                                                                                              ctx->d_newcnt);
         });
     if (n)
-        push_k<<<(n + 255) / 256, 256, 0, ctx->stream>>>(n, task ? ctx->d_push_task : nullptr, first_handle, ctx->d_push_cls,
+        push_k<<<(n + 255) / 256, 256, 0, ctx->stream>>>(n, task ? (u32*)ctx->d_push_task : nullptr, first_handle, ctx->d_push_cls,
                                                          ctx->d_push_prio, ctx->d_key, ctx->d_prio, ctx->d_levels,
                                                          (u32)ctx->dev_levels.size(), ctx->coarse ? 1 : 0, ctx->d_newcnt, ctx->d_newprio);
     ctx->stats.kernel_launches += n ? 2 : 0;
@@ -1419,15 +1382,15 @@ int hqs_dag_load(hqs_ctx* ctx, uint32_t n_tasks, const uint32_t* class_id, const
     CU(cudaSetDevice(ctx->device));
     int rc = ensure_handles(ctx, n_tasks);
     if (rc) return rc;
-    CU(cudaStreamSynchronize(ctx->stream));
-    if (ctx->d_deps) { CU(cudaFree(ctx->d_deps)); ctx->d_deps = nullptr; }
-    if (ctx->d_cons_off) { CU(cudaFree(ctx->d_cons_off)); ctx->d_cons_off = nullptr; }
-    if (ctx->d_cons) { CU(cudaFree(ctx->d_cons)); ctx->d_cons = nullptr; }
-    u32* d_cls = nullptr;
-    CU(cudaMalloc(&ctx->d_deps, (size_t)n_tasks * 4));
-    CU(cudaMalloc(&ctx->d_cons_off, ((size_t)n_tasks + 1) * 4));
-    CU(cudaMalloc(&ctx->d_cons, std::max<size_t>(n_edges, 1) * 4));
-    CU(cudaMalloc(&d_cls, (size_t)n_tasks * 4));
+    CU(cudaStreamSynchronize(ctx->stream));       // an earlier DAG's arrays are freed below
+    Buf<u32> dev_deps, dev_off, dev_cons, d_cls;
+    CU(dev_deps.grow(n_tasks, ctx->stream));
+    CU(dev_off.grow((size_t)n_tasks + 1, ctx->stream));
+    CU(dev_cons.grow(std::max<size_t>(n_edges, 1), ctx->stream));
+    CU(d_cls.grow(n_tasks, ctx->stream));
+    ctx->d_deps = std::move(dev_deps);
+    ctx->d_cons_off = std::move(dev_off);
+    ctx->d_cons = std::move(dev_cons);
     CU(cudaMemsetAsync(ctx->d_key, 0, (size_t)ctx->cap_handles * 4, ctx->stream));
     CU(cudaMemcpyAsync(ctx->d_deps, n_deps, (size_t)n_tasks * 4, cudaMemcpyHostToDevice, ctx->stream));
     CU(cudaMemcpyAsync(ctx->d_cons_off, cons_off, ((size_t)n_tasks + 1) * 4, cudaMemcpyHostToDevice, ctx->stream));
@@ -1438,7 +1401,7 @@ int hqs_dag_load(hqs_ctx* ctx, uint32_t n_tasks, const uint32_t* class_id, const
     distinct_priorities(priority, n_tasks, fresh);
     ctx->levels.clear();
     merge_levels(ctx, fresh);
-    if ((rc = upload_levels(ctx))) { cudaFree(d_cls); return rc; }
+    if ((rc = upload_levels(ctx))) return rc;
     ctx->n_handles = n_tasks;
     ctx->stats.n_handles = n_tasks;
     dag_init_k<<<(n_tasks + 255) / 256, 256, 0, ctx->stream>>>(n_tasks, d_cls, ctx->d_prio, ctx->d_deps, ctx->d_key,
@@ -1447,7 +1410,6 @@ int hqs_dag_load(hqs_ctx* ctx, uint32_t n_tasks, const uint32_t* class_id, const
     ctx->stats.kernel_launches++;
     CU(cudaGetLastError());
     CU(cudaStreamSynchronize(ctx->stream));
-    CU(cudaFree(d_cls));
     ctx->dag = true;
     return HQS_OK;
 }
@@ -1545,8 +1507,8 @@ int graph_compact(hqs_ctx* ctx, u32 n_edges) {
     }
     const u64 want = std::max<u64>(ctx->pool_cap, 2ull * live + n_edges);
     if (want >= GRAPH_NIL) return fail(ctx, HQS_E_LIMIT, "the edge pool would need %llu slots", (unsigned long long)want);
-    GraphEdge* fresh = nullptr;
-    CU(cudaMalloc(&fresh, (size_t)want * sizeof(GraphEdge)));
+    Buf<GraphEdge> fresh;
+    CU(fresh.grow(want, ctx->stream));
     if (nb) {
         graph_dispatch(ctx->shard_graph, [&](auto S) {
             graph_gc_move_k<decltype(S)::value><<<nb, GRAPH_NT, 0, ctx->stream>>>(nh, ctx->d_ghead, ctx->d_pool, fresh, gk,
@@ -1556,8 +1518,7 @@ int graph_compact(hqs_ctx* ctx, u32 n_edges) {
         CU(cudaGetLastError());
     }
     CU(cudaStreamSynchronize(ctx->stream));
-    CU(cudaFree(ctx->d_pool));
-    ctx->d_pool = fresh;
+    ctx->d_pool = std::move(fresh);
     ctx->pool_cap = (u32)want;
     ctx->pool_used = live;
     ctx->pool_compactions++;
@@ -1675,11 +1636,7 @@ int graph_push_impl(hqs_ctx* ctx, u32 n, const u32* task, const u32* class_id, c
     if ((rc = ensure_graph_storage(ctx))) return rc;
     // d_gstage: offsets, dependencies, then (sharded) the batch's global handles
     const size_t stage = (size_t)n + 1 + me + (shard ? n : 0);
-    if (stage > ctx->gstage_cap) {
-        const size_t cap = std::max<size_t>(stage * 2, 1u << 16);
-        if ((rc = dev_realloc(ctx, &ctx->d_gstage, 0, cap, false, false))) return rc;
-        ctx->gstage_cap = cap;
-    }
+    if (stage > ctx->d_gstage.size()) CU(ctx->d_gstage.grow(std::max<size_t>(stage * 2, 1u << 16), ctx->stream));
     // pageable sources: staged by the runtime before the calls return
     CU(cudaMemcpyAsync(ctx->d_gstage, off.data(), ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, ctx->stream));
     if (me) CU(cudaMemcpyAsync(ctx->d_gstage + n + 1, dep.data(), (size_t)me * 4, cudaMemcpyHostToDevice, ctx->stream));
@@ -1694,7 +1651,7 @@ int graph_push_impl(hqs_ctx* ctx, u32 n, const u32* task, const u32* class_id, c
     if (!ctx->d_pool) {
         const u64 cap = std::max<u64>(2ull * me, GRAPH_POOL_MIN);
         if (cap >= GRAPH_NIL) return fail(ctx, HQS_E_LIMIT, "the edge pool would need %llu slots", (unsigned long long)cap);
-        CU(cudaMalloc(&ctx->d_pool, (size_t)cap * sizeof(GraphEdge)));
+        CU(ctx->d_pool.grow(cap, ctx->stream));
         ctx->pool_cap = (u32)cap;
         ctx->pool_used = 0;
     } else if ((u64)ctx->pool_used + me > ctx->pool_cap) {
@@ -1861,27 +1818,25 @@ int hqs_graph_debug(hqs_ctx* ctx, uint64_t out[4]) {
     if (int rc = ctx->shard_graph ? shard_graph_mode_check(ctx, "hqs_graph_debug") : graph_mode_check(ctx, "hqs_graph_debug"))
         return rc;
     CU(cudaSetDevice(ctx->device));
-    unsigned long long* d_out = nullptr;
-    CU(cudaMalloc(&d_out, 2 * sizeof(unsigned long long)));
+    Buf<unsigned long long> d_out;
+    CU(d_out.grow(2, ctx->stream));
     unsigned long long h[2] = {0, 0};
-    cudaError_t e = cudaMemsetAsync(d_out, 0, sizeof h, ctx->stream);
-    if (e == cudaSuccess && ctx->shard_graph) {
+    CU(cudaMemsetAsync(d_out, 0, sizeof h, ctx->stream));
+    if (ctx->shard_graph) {
         // the replicated lists over the global handles, the waiting tasks over the own keys
         graph_debug_k<<<(ctx->g_total + 255) / 256, 256, 0, ctx->stream>>>(ctx->g_total, nullptr, ctx->d_ghead, ctx->d_pool, d_out);
         if (ctx->n_handles)
             graph_debug_k<<<(ctx->n_handles + 255) / 256, 256, 0, ctx->stream>>>(ctx->n_handles, ctx->d_key, nullptr, nullptr, d_out);
         ctx->stats.kernel_launches += ctx->n_handles ? 2 : 1;
-        e = cudaGetLastError();
-    } else if (e == cudaSuccess && ctx->n_handles) {
+        CU(cudaGetLastError());
+    } else if (ctx->n_handles) {
         graph_debug_k<<<(ctx->n_handles + 255) / 256, 256, 0, ctx->stream>>>(ctx->n_handles, ctx->d_key,
-                                                                           ctx->graph_storage ? ctx->d_ghead : nullptr, ctx->d_pool, d_out);
+                                                                           ctx->graph_storage ? (u32*)ctx->d_ghead : nullptr, ctx->d_pool, d_out);
         ctx->stats.kernel_launches++;
-        e = cudaGetLastError();
+        CU(cudaGetLastError());
     }
-    if (e == cudaSuccess) e = cudaMemcpyAsync(h, d_out, sizeof h, cudaMemcpyDeviceToHost, ctx->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-    cudaFree(d_out);
-    if (e != cudaSuccess) return fail(ctx, HQS_E_CUDA, "hqs_graph_debug: %s", cudaGetErrorString(e));
+    CU(cudaMemcpyAsync(h, d_out, sizeof h, cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
     out[0] = h[0];
     out[1] = ctx->pool_cap;
     out[2] = ctx->pool_compactions;
@@ -1906,10 +1861,7 @@ int hqs_shard_graph_init(hqs_ctx* ctx, uint32_t n_total, uint32_t lo, uint32_t h
             if (k & KEY_VALID) return fail(ctx, HQS_E_STATE, "the task table already holds a live task");
     }
     const u32 cap = (n_total + 1023u) & ~1023u;
-    u32* gvalid = nullptr;
-    CU(cudaMalloc(&gvalid, (size_t)cap / 8));
-    CU(cudaMemsetAsync(gvalid, 0, (size_t)cap / 8, ctx->stream));
-    ctx->d_gvalid = gvalid;
+    CU(ctx->d_gvalid.grow(cap / 32, ctx->stream, false, 0));
     ctx->shard_graph = true;
     ctx->g_total = n_total;
     ctx->g_lo = lo;
@@ -2004,7 +1956,7 @@ int hqs_grouped_reserve(hqs_ctx* ctx, uint32_t n_workers, uint32_t out_cap) {
     if (!ctx) return HQS_E_INVALID;
     if (n_workers == 0 || n_workers > HQS_MAX_WORKERS) return fail(ctx, HQS_E_LIMIT, "n_workers=%u outside 1..%u", n_workers, HQS_MAX_WORKERS);
     CU(cudaSetDevice(ctx->device));
-    int rc = ensure_group_buffers(ctx, n_workers, std::max(out_cap, ctx->out_cap_dev));
+    int rc = ensure_group_buffers(ctx, n_workers, std::max(out_cap, (u32)ctx->d_out.size()));
     if (rc) return rc;
     CU(cudaStreamSynchronize(ctx->stream));
     return HQS_OK;
@@ -2046,7 +1998,7 @@ int hqs_query_fetch(hqs_ctx* ctx, uint32_t* n_would_assign, uint32_t* per_worker
     TickHeaderOut hdr;
     const int rc = wait_header(ctx, &hdr);
     if (rc) return rc;
-    if (free_after) memcpy(free_after, ctx->h_hdr + sizeof(TickHeaderOut), (size_t)ctx->last_W * ctx->R * 8);
+    if (free_after) memcpy(free_after, ctx->tick.h_hdr + sizeof(TickHeaderOut), (size_t)ctx->last_W * ctx->R * 8);
     // the count segments cover every group's assigned ranks [0, k), so the per-worker counts sum to the tasks assigned over
     // all ranks; the header's n_assigned of a sharded launch is this rank's share only (the solver's local output offsets)
     u32 total = 0;
@@ -2129,10 +2081,14 @@ int hqs_shard_xbuf(hqs_ctx* ctx, void** d_xbuf, uint8_t ipc_handle[HQS_IPC_HANDL
     if (!ctx) return HQS_E_INVALID;
     CU(cudaSetDevice(ctx->device));
     if (!ctx->d_xbuf) {
-        CU(cudaMalloc(&ctx->d_xbuf, xbuf_bytes()));
-        CU(cudaMemset(ctx->d_xbuf, 0, xbuf_bytes()));
-        CU(cudaMalloc(&ctx->d_xall, HQS_MAX_GROUPS * sizeof(u32)));
-        CU(cudaMalloc(&ctx->d_xbefore, HQS_MAX_GROUPS * sizeof(u32)));
+        Buf<u32> xbuf, xall, xbefore;
+        CU(xbuf.grow(xbuf_bytes() / sizeof(u32), ctx->stream));
+        CU(cudaMemset(xbuf, 0, xbuf_bytes()));
+        CU(xall.grow(HQS_MAX_GROUPS, ctx->stream));
+        CU(xbefore.grow(HQS_MAX_GROUPS, ctx->stream));
+        ctx->d_xbuf = std::move(xbuf);
+        ctx->d_xall = std::move(xall);
+        ctx->d_xbefore = std::move(xbefore);
     }
     if (d_xbuf) *d_xbuf = ctx->d_xbuf;
     if (ipc_handle) {
@@ -2224,7 +2180,8 @@ int hqs_shard_query_solve(hqs_ctx* ctx, const uint32_t* d_counts_all) {
 int hqs_device_result(hqs_ctx* ctx, const hqs_assignment** d_out, const uint32_t** d_out_n) {
     if (!ctx) return HQS_E_INVALID;
     if (d_out) *d_out = ctx->d_out;
-    if (d_out_n) *d_out_n = ctx->d_hdr ? &ctx->d_hdr->n_assigned : nullptr;
+    TickHeaderOut* hdr = ctx->tick.hdr;
+    if (d_out_n) *d_out_n = hdr ? &hdr->n_assigned : nullptr;
     return HQS_OK;
 }
 
