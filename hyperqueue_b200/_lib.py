@@ -31,7 +31,7 @@ ABI_SYMBOLS = [
     "hqs_levels_live", "hqs_levels_retain",
     "hqs_graph_push", "hqs_graph_finished", "hqs_graph_cancel", "hqs_graph_debug",
     "hqs_shard_graph_init", "hqs_shard_graph_push", "hqs_shard_graph_finished", "hqs_shard_graph_cancel",
-    "hqs_shard_graph_remove",
+    "hqs_shard_graph_remove", "hqs_handles_compact",
 ]
 HQS_IPC_HANDLE_BYTES = 64
 
@@ -101,6 +101,8 @@ def load_shim() -> C.CDLL:
         _shim.hqshim_selftest_graph.restype = C.c_int
         _shim.hqshim_selftest_graph_cancel.argtypes = [C.c_int, C.c_int]
         _shim.hqshim_selftest_graph_cancel.restype = C.c_int
+        _shim.hqshim_selftest_retire.argtypes = [C.c_int, C.c_int]
+        _shim.hqshim_selftest_retire.restype = C.c_int
         _shim.hqshim_time_mapping.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_int,
                                               C.c_uint32, C.c_void_p, C.POINTER(C.c_uint64)]
         _shim.hqshim_time_mapping.restype = C.c_int
@@ -133,6 +135,7 @@ def load_library() -> C.CDLL:
     lib.hqs_graph_finished.argtypes = [vp, u32, u32p, C.POINTER(C.POINTER(C.c_uint32)), C.POINTER(C.c_uint32)]
     lib.hqs_graph_cancel.argtypes = [vp, u32, u32p, C.POINTER(C.POINTER(C.c_uint32)), C.POINTER(C.c_uint32)]
     lib.hqs_graph_debug.argtypes = [vp, C.POINTER(C.c_uint64)]
+    lib.hqs_handles_compact.argtypes = [vp, u32, u32p, C.POINTER(C.POINTER(C.c_uint32)), C.POINTER(C.c_uint32)]
     lib.hqs_shard_graph_init.argtypes = [vp, u32, u32, u32]
     lib.hqs_shard_graph_push.argtypes = [vp, u32, u32p, u32p, u64p, u32p, u32p, C.POINTER(C.c_uint32)]
     lib.hqs_shard_graph_finished.argtypes = [vp, u32, u32p, C.POINTER(C.POINTER(C.c_uint32)), C.POINTER(C.c_uint32)]

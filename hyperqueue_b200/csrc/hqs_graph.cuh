@@ -277,12 +277,17 @@ __global__ void __launch_bounds__(GRAPH_NT) graph_gc_count_k(u32 n_handles, cons
     if (threadIdx.x == 0) blk[blockIdx.x] = sum;
 }
 
-// pass 2 (blk scanned): every list is rewritten, in its order, into consecutive slots of the fresh pool
-template <bool S>
+// pass 2 (blk scanned): every list is rewritten, in its order, into consecutive slots of the fresh pool.
+// RN (hqs_handles_compact): the handles are renumbered as well.  Every consumer and every producer with a non-empty list is
+// VALID, so it survives, and new_of_old[] holds its new handle: the edges take the new consumer handles, and each non-empty
+// list's head goes to head_out[new handle] (a fresh array; ghead is only read).
+template <bool S, bool RN = false>
 __global__ void __launch_bounds__(GRAPH_NT) graph_gc_move_k(u32 n_handles, u32* __restrict__ ghead,
                                                              const GraphEdge* __restrict__ pool, GraphEdge* __restrict__ fresh,
                                                              const GraphKeys k, const u32* __restrict__ gdeps,
-                                                             const u32* __restrict__ ggen, const u32* __restrict__ blk) {
+                                                             const u32* __restrict__ ggen, const u32* __restrict__ blk,
+                                                             const u32* __restrict__ new_of_old = nullptr,
+                                                             u32* __restrict__ head_out = nullptr) {
     const u32 h0 = (blockIdx.x * GRAPH_NT + threadIdx.x) * GRAPH_PER_THREAD;
     u32 c = 0;
     for (u32 j = 0; j < GRAPH_PER_THREAD; ++j) {
@@ -298,11 +303,12 @@ __global__ void __launch_bounds__(GRAPH_NT) graph_gc_move_k(u32 n_handles, u32* 
         for (u32 e = ghead[h]; e != GRAPH_NIL; e = pool[e].next) {
             const GraphEdge E = pool[e];
             if (!graph_edge_waits<S>(E, k, gdeps, ggen)) continue;
-            fresh[pos] = GraphEdge{E.cons, E.gen, GRAPH_NIL};
+            fresh[pos] = GraphEdge{RN ? new_of_old[E.cons] : E.cons, E.gen, GRAPH_NIL};
             if (prev == GRAPH_NIL) first = pos; else fresh[prev].next = pos;
             prev = pos++;
         }
-        ghead[h] = first;
+        if (!RN) ghead[h] = first;
+        else if (first != GRAPH_NIL) head_out[new_of_old[h]] = first;
     }
 }
 
@@ -477,5 +483,34 @@ __global__ void graph_cancel_apply_k(u32* __restrict__ work, const GraphCancelSy
         if (u32* kh = graph_own<S>(k, h)) *kh &= ~(KEY_READY | KEY_VALID | KEY_DONE | KEY_PF);
         if (S) atomicAnd(&k.gvalid[h >> 5], ~(1u << (h & 31)));
         ghead[h] = GRAPH_NIL;
+    }
+}
+
+// hqs_handles_compact: the survivors (VALID keys, plus the handles named in keep) are marked in a zeroed bitmap of one bit
+// per handle; the ordered compaction above then writes them out ascending.  One thread per handle (a warp covers one bitmap
+// word) and one per keep entry.
+__global__ void compact_mark_k(u32 n_handles, const u32* __restrict__ key, u32 n_keep, const u32* __restrict__ keep,
+                               u32* __restrict__ bits) {
+    const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
+    const u32 m = __ballot_sync(0xffffffffu, i < n_handles && (key[i] & KEY_VALID));
+    if ((threadIdx.x & 31) == 0 && m) atomicOr(&bits[i >> 5], m);
+    if (i < n_keep) atomicOr(&bits[keep[i] >> 5], 1u << (keep[i] & 31));      // host-checked: keep[i] < n_handles
+}
+
+// survivor i (old handle order[i]) becomes handle i: its key and priority, and on a graph context its dependency count and
+// incarnation, move to slot i of the fresh arrays; new_of_old[old] = i for the edge rewrite (graph_gc_move_k<S, true>)
+__global__ void compact_gather_k(u32 n_kept, const u32* __restrict__ order, const u32* __restrict__ key,
+                                 const u64* __restrict__ prio, const u32* __restrict__ gdeps, const u32* __restrict__ ggen,
+                                 u32* __restrict__ key_out, u64* __restrict__ prio_out, u32* __restrict__ gdeps_out,
+                                 u32* __restrict__ ggen_out, u32* __restrict__ new_of_old) {
+    const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_kept) return;
+    const u32 o = order[i];
+    key_out[i] = key[o];
+    prio_out[i] = prio[o];
+    new_of_old[o] = i;
+    if (gdeps) {
+        gdeps_out[i] = gdeps[o];
+        ggen_out[i] = ggen[o];
     }
 }

@@ -1783,6 +1783,81 @@ int graph_cancel_impl(hqs_ctx* ctx, u32 n, const u32* task, const u32** cancelle
     if (n_cancelled) *n_cancelled = (u32)(last - first);
     return HQS_OK;
 }
+
+// The body of hqs_handles_compact, after the checks (keep staged at d_push_task).  Nothing of the context is written
+// before the end: the survivors are gathered into fresh arrays, the edges into a fresh pool, and these replace the
+// context's arrays only once every kernel and copy has succeeded.
+int handles_compact_impl(hqs_ctx* ctx, u32 n_keep) {
+    const u32 nh = ctx->n_handles, cap = ctx->cap_handles;
+    const u32 n_words = (nh + 31) / 32;
+    const u32 nb_words = (n_words + GRAPH_PER_BLOCK - 1) / GRAPH_PER_BLOCK;   // ordered emit over the bitmap
+    const u32 nb_lists = (nh + GRAPH_PER_BLOCK - 1) / GRAPH_PER_BLOCK;        // edge rewrite over the producers
+    const bool graph = ctx->graph_storage;
+    const bool edges = graph && ctx->d_pool;
+    cudaStream_t s = ctx->stream;
+    Buf<u32> bits, order, new_of_old, blk, key, gdeps, ggen, ghead;
+    Buf<u64> prio;
+    Buf<GraphEdge> pool;
+    CU(bits.grow(n_words, s, false, 0));
+    CU(order.grow(nh, s));
+    CU(new_of_old.grow(nh, s));
+    CU(blk.grow((size_t)std::max(nb_words, nb_lists) + 2, s));     // per-block sums, then the two totals
+    CU(key.grow(cap, s, false, 0));
+    CU(prio.grow(cap, s, false, 0));
+    if (graph) {
+        CU(gdeps.grow(cap, s, false, 0));
+        CU(ggen.grow(cap, s, false, 0));
+        CU(ghead.grow(cap, s, false, 0xFF));
+    }
+    if (edges) CU(pool.grow(ctx->pool_cap, s));
+    u32* total = blk + std::max(nb_words, nb_lists);                // [0] survivors, [1] live edges
+    CU(cudaMemsetAsync(total, 0, 2 * sizeof(u32), s));
+    const u32 nt = std::max(nh, n_keep);
+    compact_mark_k<<<(nt + 255) / 256, 256, 0, s>>>(nh, ctx->d_key, n_keep, ctx->d_push_task, bits);
+    graph_ready_count_k<<<nb_words, GRAPH_NT, 0, s>>>(n_words, bits, blk);
+    graph_scan_k<<<1, 1024, 0, s>>>(nb_words, blk, total);
+    graph_ready_emit_k<<<nb_words, GRAPH_NT, 0, s>>>(n_words, bits, blk, order);
+    ctx->stats.kernel_launches += 4;
+    const GraphKeys gk = graph_keys(ctx);
+    if (edges) {
+        graph_gc_count_k<false><<<nb_lists, GRAPH_NT, 0, s>>>(nh, ctx->d_ghead, ctx->d_pool, gk, ctx->d_gdeps, ctx->d_ggen, blk);
+        graph_scan_k<<<1, 1024, 0, s>>>(nb_lists, blk, total + 1);
+        ctx->stats.kernel_launches += 2;
+    }
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(ctx->h_small + 4, total, 2 * sizeof(u32), cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    const u32 n_kept = ctx->h_small[4], live = ctx->h_small[5];
+    if (n_kept) {
+        compact_gather_k<<<(n_kept + 255) / 256, 256, 0, s>>>(n_kept, order, ctx->d_key, ctx->d_prio,
+                                                              graph ? (u32*)ctx->d_gdeps : nullptr, ctx->d_ggen, key, prio,
+                                                              gdeps, ggen, new_of_old);
+        ctx->stats.kernel_launches++;
+    }
+    if (edges) {
+        graph_gc_move_k<false, true><<<nb_lists, GRAPH_NT, 0, s>>>(nh, ctx->d_ghead, ctx->d_pool, pool, gk, ctx->d_gdeps,
+                                                                    ctx->d_ggen, blk, new_of_old, ghead);
+        ctx->stats.kernel_launches++;
+    }
+    CU(cudaGetLastError());
+    ctx->g_new_ready.resize(n_kept);
+    if (n_kept) CU(cudaMemcpyAsync(ctx->g_new_ready.data(), order, (size_t)n_kept * 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    ctx->d_key = std::move(key);
+    ctx->d_prio = std::move(prio);
+    if (graph) {
+        ctx->d_gdeps = std::move(gdeps);
+        ctx->d_ggen = std::move(ggen);
+        ctx->d_ghead = std::move(ghead);
+    }
+    if (edges) {
+        ctx->d_pool = std::move(pool);
+        ctx->pool_used = live;
+    }
+    ctx->n_handles = n_kept;
+    ctx->stats.n_handles = n_kept;
+    return HQS_OK;
+}
 }  // namespace
 
 extern "C" {
@@ -1841,6 +1916,34 @@ int hqs_graph_debug(hqs_ctx* ctx, uint64_t out[4]) {
     out[1] = ctx->pool_cap;
     out[2] = ctx->pool_compactions;
     out[3] = h[1];
+    return HQS_OK;
+}
+
+int hqs_handles_compact(hqs_ctx* ctx, uint32_t n_keep, const uint32_t* keep, const uint32_t** old_of_new, uint32_t* n_kept) {
+    if (!ctx) return HQS_E_INVALID;
+    ctx->g_new_ready.clear();
+    if (old_of_new) *old_of_new = ctx->g_new_ready.data();
+    if (n_kept) *n_kept = 0;
+    if (ctx->dag) return fail(ctx, HQS_E_STATE, "hqs_handles_compact is not available after hqs_dag_load");
+    if (ctx->x_world) return fail(ctx, HQS_E_STATE, "hqs_handles_compact is not available on a sharded ready set");
+    if (ctx->shard_graph) return fail(ctx, HQS_E_STATE, "hqs_handles_compact is not available on a sharded graph context");
+    if (ctx->tick_pending) return fail(ctx, HQS_E_STATE, "the previous tick has not been fetched");
+    if (n_keep && !keep) return fail(ctx, HQS_E_INVALID, "null keep array");
+    for (u32 i = 0; i < n_keep; ++i)
+        if (keep[i] >= ctx->n_handles)
+            return fail(ctx, HQS_E_INVALID, "keep handle %u >= n_handles %u (nothing was compacted)", keep[i], ctx->n_handles);
+    if (!ctx->n_handles) return HQS_OK;
+    CU(cudaSetDevice(ctx->device));
+    if (int rc = ensure_push_staging(ctx, n_keep)) return rc;
+    if (n_keep) CU(cudaMemcpyAsync(ctx->d_push_task, keep, (size_t)n_keep * 4, cudaMemcpyHostToDevice, ctx->stream));
+    const int rc = handles_compact_impl(ctx, n_keep);
+    if (rc) {
+        ctx->g_new_ready.clear();
+        cudaStreamSynchronize(ctx->stream);       // the caller may free keep as soon as we return
+        return rc;
+    }
+    if (old_of_new) *old_of_new = ctx->g_new_ready.data();
+    if (n_kept) *n_kept = (u32)ctx->g_new_ready.size();
     return HQS_OK;
 }
 

@@ -127,6 +127,8 @@ size_t GpuCore::n_waiting() const {
 uint32_t GpuCore::handle_of(TaskId task) {
     auto it = handle_of_.find(task.as_u64());
     if (it != handle_of_.end()) return it->second;
+    if (tasks_.size() >= handle_end_)       // handle 0xFFFFFFFF is reserved: a wrap would alias a live task's handle
+        throw std::length_error("the task handle space is exhausted: retire the handles of forgotten tasks (retire_handles)");
     const uint32_t h = (uint32_t)tasks_.size();
     tasks_.emplace_back();
     tasks_[h].id = task;
@@ -363,6 +365,7 @@ void GpuCore::on_task_finished(TaskId task) {
     }
     t.worker = -1;
     t.live = false;
+    t.forgotten = true;
     forget_h_.push_back(it->second);
 }
 

@@ -62,6 +62,7 @@ int64_t GpuCore::leave_worker(TaskState& t) {
     t.retracting_from = -1;
     t.live = false;
     t.waiting = false;
+    t.forgotten = true;
     return to;
 }
 
@@ -82,6 +83,7 @@ CancelledTasks GpuCore::on_cancel_tasks(const std::vector<TaskId>& tasks) {
     }
     for (uint32_t h : cancel_on_device(named)) {
         tasks_[h].live = tasks_[h].waiting = false;             // consumers: waiting, so held by no worker
+        tasks_[h].forgotten = true;
         left.insert(h);
     }
     for (uint32_t h : left) out.cancelled.push_back(tasks_[h].id);
@@ -101,6 +103,7 @@ std::vector<TaskId> GpuCore::on_task_failed(TaskId task) {
     for (uint32_t c : cancel_on_device({h}))
         if (c != h) {
             tasks_[c].live = tasks_[c].waiting = false;
+            tasks_[c].forgotten = true;
             consumers.push_back(tasks_[c].id);
         }
     std::sort(consumers.begin(), consumers.end());

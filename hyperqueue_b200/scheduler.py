@@ -653,6 +653,50 @@ class GpuScheduler:
         gone = np.ctypeslib.as_array(ptr, shape=(k.value,)).copy() if k.value else np.zeros(0, dtype=np.uint32)
         return gone, cancel_bookkeeping(self, h, gone)
 
+    def compact_handles(self, keep=None) -> np.ndarray:
+        """Retires the handles of forgotten tasks (hqs_handles_compact): the surviving handles are renumbered 0 ..
+        n_kept - 1 in ascending order, so handle order stays TaskId order and a long-running server's tick cost and memory
+        follow its live tasks.  A handle survives if its task is in the device table (waiting, ready, prefilled, assigned
+        and not finished or removed), if this object still tracks it (assigned to a worker, prefilled, or with a pending
+        redirect or retract), or if it is in `keep` (handles the caller tracks).  A finished task stays in the table until
+        the caller retires it with remove_ready_tasks (tasks_finished does not take it out).  The host mirror is renumbered
+        with the table.  Returns old_of_new: the old handle of each new handle, ascending; the caller renumbers its own
+        handles with it (np.searchsorted(old_of_new, old) for a survivor)."""
+        n = int(self._lib_stats().n_handles)
+        tracked = np.zeros(0, dtype=np.int64)
+        if n:
+            m = min(n, self._task_worker.shape[0])
+            tracked = np.nonzero((self._task_worker[:m] >= 0) | (self._pf_worker[:m] >= 0))[0]
+        extra = list(self.redirects.keys()) + list(self._retracting_from.keys())
+        k = np.concatenate([tracked, np.asarray(extra, dtype=np.int64),
+                            np.zeros(0, np.int64) if keep is None else np.asarray(keep, dtype=np.int64).ravel()])
+        k = np.ascontiguousarray(np.unique(k), dtype=np.uint32)
+        ptr = C.POINTER(C.c_uint32)()
+        nk = C.c_uint32(0)
+        self._check(self._lib.hqs_handles_compact(self._ctx, k.size, L.ptr(k) if k.size else None, C.byref(ptr),
+                                                  C.byref(nk)))
+        old_of_new = np.ctypeslib.as_array(ptr, shape=(nk.value,)).copy() if nk.value else np.zeros(0, dtype=np.uint32)
+        kept = old_of_new.astype(np.int64)
+        self._grow_tasks(n)
+
+        def remap(a: np.ndarray, fill) -> np.ndarray:
+            out = np.full_like(a, fill)
+            out[: kept.size] = a[kept]
+            return out
+
+        self._task_class = remap(self._task_class, 0)
+        self._task_worker = remap(self._task_worker, -1)
+        self._task_variant = remap(self._task_variant, 0)
+        self._task_prio = remap(self._task_prio, 0)
+        self._pf_worker = remap(self._pf_worker, -1)
+
+        def new_of(t: int) -> int:
+            return int(np.searchsorted(old_of_new, t))
+
+        self.redirects = {new_of(t): v for t, v in self.redirects.items()}
+        self._retracting_from = {new_of(t): v for t, v in self._retracting_from.items()}
+        return old_of_new
+
     def graph_debug(self) -> np.ndarray:
         """hqs_graph_debug: [live edges, edge-pool capacity, pool compactions, waiting tasks]."""
         out = (C.c_uint64 * 4)()

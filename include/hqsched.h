@@ -226,6 +226,29 @@ int hqs_graph_finished(hqs_ctx* ctx, uint32_t n, const uint32_t* task, const uin
 int hqs_graph_cancel(hqs_ctx* ctx, uint32_t n, const uint32_t* task, const uint32_t** cancelled, uint32_t* n_cancelled);
 int hqs_graph_debug(hqs_ctx* ctx, uint64_t out[4]);
 
+/* Retires the handles of forgotten tasks: an order-preserving renumbering of the task table, so that a long-running server's
+ * tick cost and memory follow its live tasks, not every task it has ever seen.
+ * Survivors: every handle whose key is VALID (waiting, ready, prefilled, or assigned and not finished or removed), plus the
+ * handles named in keep[0 .. n_keep).  keep may name handles in any state, in any order, and more than once; the host names
+ * there the tasks it still tracks that have left the table (for example a prefilled task a worker started, which
+ * hqs_ready_remove took out).
+ * Renumbering: survivor i, in ascending old handle, becomes handle i, so handle order stays TaskId order and new handles
+ * keep being appended after the survivors.  *old_of_new points to the *n_kept old handles, ascending, in the buffer
+ * hqs_graph_finished uses, valid until the next call on the context.  n_handles (and hqs_stats.n_handles) becomes n_kept.
+ * What moves with a survivor: its key verbatim (READY, DONE, VALID and PREFILLED bits, level and class), its priority and,
+ * on a graph context, its dependency count, its incarnation and its consumer list, with the consumers renumbered.  An edge
+ * whose consumer no longer waits on the edge's incarnation is dropped, as a pool compaction drops it.
+ * The slots [n_kept, old n_handles) become slots that were never used: key 0, no dependencies, incarnation 0, an empty
+ * consumer list.  Capacity is kept.  The level table, the class table, the prefill configuration and the prefill mask given
+ * with hqs_prefill_state are unchanged.
+ * HQS_E_INVALID with nothing changed: a keep entry >= n_handles, or keep == NULL with n_keep > 0.  HQS_E_STATE with nothing
+ * changed: a tick or query is pending, after hqs_dag_load, on a context attached with hqs_shard_attach or set up with
+ * hqs_shard_graph_init.  A failed allocation or CUDA error (HQS_E_CUDA) leaves the context as it was: the survivors are
+ * gathered into fresh arrays that replace the table only at the end.
+ * The number of kernel launches does not depend on n_handles (at most eight); the call synchronises with the host twice
+ * (the survivor count, then the copy of *old_of_new) and does no per-handle work on the host. */
+int hqs_handles_compact(hqs_ctx* ctx, uint32_t n_keep, const uint32_t* keep, const uint32_t** old_of_new, uint32_t* n_kept);
+
 /* Task graphs over a sharded ready set: the graph is replicated on every rank, each task's key lives on its owner.
  * hqs_shard_graph_init: this context owns the GLOBAL handles [lo, hi) of a graph over n_total handles (its key table holds
  * handle h at h - lo, as in the sharded tick) and allocates the replicated graph (the three per-handle arrays and the work

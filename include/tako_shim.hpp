@@ -146,6 +146,17 @@ public:
     // returns its transitive consumers, ascending TaskId (the list tako hands to on_task_error), which left with it.
     std::vector<TaskId> on_task_failed(TaskId task);
 
+    // Retires the handles of the tasks tako has forgotten (finished, or cancelled or failed with their consumers): pending
+    // submits and finishes are flushed, the device table is renumbered in TaskId order without them (hqs_handles_compact) and
+    // the host mirror with it.  Every other task keeps a handle, whatever its state.  Returns the number of handles retired.
+    // The embedding server decides when, for example when n_handles() exceeds twice the tasks it knows.  Defined in
+    // tako_shim_retire.cpp.
+    size_t retire_handles();
+    size_t n_handles() const { return tasks_.size(); }   // handles given out and not retired
+    // Test aid: handle_of throws std::length_error once `end` handles are in use (default: the whole 32-bit space, less
+    // 0xFFFFFFFF, which the C ABI reserves).
+    void limit_handles_for_testing(uint32_t end) { handle_end_ = end; }
+
     // SchedulerConfig::proactive_filling_reserve / _max (scheduler/state.rs:14-21).  tako's defaults are 16 / 40; this
     // class starts with proactive filling OFF (max = 0) and the embedding server switches it on.
     void set_scheduler_config(uint32_t proactive_filling_reserve, uint32_t proactive_filling_max);
@@ -179,6 +190,7 @@ private:
         bool waiting = false;             // submitted with a dependency that has not finished yet
         int64_t prefilled_on = -1;        // TaskRuntimeState::Prefilled{worker_id}
         int64_t retracting_from = -1;     // TaskRuntimeState::Retracting{worker_id}
+        bool forgotten = false;           // finished, or cancelled / failed: tako no longer knows it (retire_handles)
     };
     struct TickInput {                    // the worker view of one tick in the C ABI's form + the free vectors it returns
         std::vector<hqs_worker> hw;
@@ -214,6 +226,7 @@ private:
     // hqs_graph_finished (both in tako_shim_graph.cpp)
     void (GpuCore::*graph_flush_)() = nullptr;
     std::vector<hqs_assignment> out_;
+    uint32_t handle_end_ = 0xFFFFFFFFu;                      // handle_of gives out handles below this
     uint32_t pf_max_ = 0;
     std::map<uint64_t, std::pair<WorkerId, ResourceVariantId>> redirects_;
     std::string last_error_;
@@ -239,6 +252,13 @@ int hqshim_selftest_graph(int device, int verbose);
 // failures of assigned tasks.  Every task runs once or is reported as left exactly once, the reported consumers equal the
 // test's own closure, and the free vectors return to the totals.  Returns the number of failed checks.
 int hqshim_selftest_graph_cancel(int device, int verbose);
+// Self-test of GpuCore::retire_handles on CUDA device `device` (tako_shim_retire.cpp): two cores get the same seeded
+// zero-duration drain of jobs with dependencies, proactive filling, cancels, failures and retract responses; one retires its
+// forgotten handles every few ticks, the other never does.  Every WorkerTaskMapping, every cancel and failure list and the
+// free vectors must be equal, and after each retire the retiring core's n_handles() must not exceed the tasks tako still
+// knows.
+// Returns the number of failed checks.
+int hqshim_selftest_retire(int device, int verbose);
 // Measuring aid (tools/grouped_probe.py): host wall time of one tick INCLUDING the construction of the per-worker lists of a
 // WorkerTaskMapping, on a context the caller has loaded (handles stand in for TaskIds).  grouped = 0: hqs_tick and one map
 // lookup + push_back per record of the flat stream; grouped = 1: hqs_tick_grouped and one lookup + reserved append per worker,
