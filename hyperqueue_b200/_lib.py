@@ -31,7 +31,7 @@ ABI_SYMBOLS = [
     "hqs_levels_live", "hqs_levels_retain",
     "hqs_graph_push", "hqs_graph_finished", "hqs_graph_cancel", "hqs_graph_debug",
     "hqs_shard_graph_init", "hqs_shard_graph_push", "hqs_shard_graph_finished", "hqs_shard_graph_cancel",
-    "hqs_shard_graph_remove", "hqs_handles_compact",
+    "hqs_shard_graph_remove", "hqs_handles_compact", "hqs_shard_graph_compact",
 ]
 HQS_IPC_HANDLE_BYTES = 64
 
@@ -141,6 +141,7 @@ def load_library() -> C.CDLL:
     lib.hqs_shard_graph_finished.argtypes = [vp, u32, u32p, C.POINTER(C.POINTER(C.c_uint32)), C.POINTER(C.c_uint32)]
     lib.hqs_shard_graph_cancel.argtypes = [vp, u32, u32p, C.POINTER(C.POINTER(C.c_uint32)), C.POINTER(C.c_uint32)]
     lib.hqs_shard_graph_remove.argtypes = [vp, u32, u32p]
+    lib.hqs_shard_graph_compact.argtypes = [vp, u32, u32p, C.POINTER(C.POINTER(C.c_uint32)), C.POINTER(C.c_uint32), u32p]
     lib.hqs_tick.argtypes = [vp, u32, vp, u64p, u64p, u8p, u32, vp, C.POINTER(C.c_uint32), u64p]
     lib.hqs_tick_launch.argtypes = [vp, u32, vp, u64p, u64p, u8p, u32]
     lib.hqs_tick_fetch.argtypes = [vp, u32, vp, C.POINTER(C.c_uint32), u64p]

@@ -514,3 +514,53 @@ __global__ void compact_gather_k(u32 n_kept, const u32* __restrict__ order, cons
         ggen_out[i] = ggen[o];
     }
 }
+
+// hqs_shard_graph_compact: the survivors are the replicated graph VALID bits plus the handles named in keep, over the global
+// handles, so every rank marks the same bitmap without reading a key.  One thread per bitmap word and one per keep entry,
+// into a zeroed bitmap.
+__global__ void shard_compact_mark_k(u32 n_words, const u32* __restrict__ gvalid, u32 n_keep, const u32* __restrict__ keep,
+                                     u32* __restrict__ bits) {
+    const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n_words && gvalid[i]) atomicOr(&bits[i], gvalid[i]);
+    if (i < n_keep) atomicOr(&bits[keep[i] >> 5], 1u << (keep[i] & 31));      // host-checked: keep[i] < n_total
+}
+
+// after the ordered emit: out[t] = the number of survivors below bound[t] (lo, then hi), by a binary search of the ascending
+// order[0 .. *n_kept).  Two threads.
+__global__ void shard_compact_range_k(const u32* __restrict__ order, const u32* __restrict__ n_kept, u32 lo, u32 hi,
+                                      u32* __restrict__ out) {
+    const u32 t = threadIdx.x;
+    if (t >= 2) return;
+    const u32 x = t ? hi : lo;
+    u32 a = 0, b = *n_kept;
+    while (a < b) {
+        const u32 m = a + (b - a) / 2;
+        if (order[m] < x) a = m + 1; else b = m;
+    }
+    out[t] = a;
+}
+
+// Survivor i (global old handle order[i]) becomes global handle i on every rank: its graph VALID bit, dependency count and
+// incarnation move to slot i of the fresh replicated arrays, and new_of_old[old] = i for the edge rewrite
+// (graph_gc_move_k<true, true>).  The rank's own survivors, i in [own_lo, own_hi), also move their key and priority from the
+// local slot old - lo to the new local slot i - own_lo (a kept handle past the old table, n_handles, has neither).  The
+// fresh bitmap is written a word per warp: blockDim is a multiple of 32, so a warp's survivors are one word's bits.
+__global__ void shard_compact_gather_k(u32 n_kept, const u32* __restrict__ order, const u32* __restrict__ gvalid,
+                                       const u32* __restrict__ gdeps, const u32* __restrict__ ggen, u32 lo, u32 n_handles,
+                                       u32 own_lo, u32 own_hi, const u32* __restrict__ key, const u64* __restrict__ prio,
+                                       u32* __restrict__ gvalid_out, u32* __restrict__ gdeps_out, u32* __restrict__ ggen_out,
+                                       u32* __restrict__ key_out, u64* __restrict__ prio_out, u32* __restrict__ new_of_old) {
+    const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
+    const u32 o = i < n_kept ? order[i] : 0u;
+    const u32 m = __ballot_sync(0xffffffffu, i < n_kept && ((gvalid[o >> 5] >> (o & 31)) & 1u));
+    if (i >= n_kept) return;
+    if ((threadIdx.x & 31) == 0) gvalid_out[i >> 5] = m;
+    gdeps_out[i] = gdeps[o];
+    ggen_out[i] = ggen[o];
+    new_of_old[o] = i;
+    if (i >= own_lo && i < own_hi) {
+        const u32 l = o - lo;
+        key_out[i - own_lo] = l < n_handles ? key[l] : 0u;
+        prio_out[i - own_lo] = l < n_handles ? prio[l] : 0ull;
+    }
+}

@@ -1858,6 +1858,92 @@ int handles_compact_impl(hqs_ctx* ctx, u32 n_keep) {
     ctx->stats.n_handles = n_kept;
     return HQS_OK;
 }
+
+// The body of hqs_shard_graph_compact, after the checks (keep staged at d_push_task).  Every rank runs the same kernels on
+// the same replicated state and the same keep list, so the replicas stay equal and every rank derives the same renumbering;
+// only the own keys differ.  As in handles_compact_impl, everything is gathered into fresh arrays that replace the context's
+// only at the end.  range receives the new owned range.
+int shard_graph_compact_impl(hqs_ctx* ctx, u32 n_keep, u32 range[2]) {
+    const u32 nt = ctx->g_total, gcap = (nt + 1023u) & ~1023u;
+    const u32 n_words = (nt + 31) / 32;
+    const u32 nb_words = (n_words + GRAPH_PER_BLOCK - 1) / GRAPH_PER_BLOCK;
+    const u32 nb_lists = (nt + GRAPH_PER_BLOCK - 1) / GRAPH_PER_BLOCK;
+    const bool edges = ctx->d_pool;
+    cudaStream_t s = ctx->stream;
+    Buf<u32> bits, order, new_of_old, blk, gvalid, gdeps, ggen, ghead, key;
+    Buf<u64> prio;
+    Buf<GraphEdge> pool;
+    CU(bits.grow(n_words, s, false, 0));
+    CU(order.grow(nt, s));
+    CU(new_of_old.grow(nt, s));
+    CU(blk.grow((size_t)std::max(nb_words, nb_lists) + 4, s));     // per-block sums, then the four totals
+    CU(gvalid.grow(gcap / 32, s, false, 0));
+    CU(gdeps.grow(gcap, s, false, 0));
+    CU(ggen.grow(gcap, s, false, 0));
+    CU(ghead.grow(gcap, s, false, 0xFF));
+    if (edges) CU(pool.grow(ctx->pool_cap, s));
+    u32* total = blk + std::max(nb_words, nb_lists);                // [0] survivors, [1] live edges, [2] new(lo), [3] new(hi)
+    CU(cudaMemsetAsync(total, 0, 4 * sizeof(u32), s));
+    const u32 nm = std::max(n_words, n_keep);
+    shard_compact_mark_k<<<(nm + 255) / 256, 256, 0, s>>>(n_words, ctx->d_gvalid, n_keep, ctx->d_push_task, bits);
+    graph_ready_count_k<<<nb_words, GRAPH_NT, 0, s>>>(n_words, bits, blk);
+    graph_scan_k<<<1, 1024, 0, s>>>(nb_words, blk, total);
+    graph_ready_emit_k<<<nb_words, GRAPH_NT, 0, s>>>(n_words, bits, blk, order);
+    shard_compact_range_k<<<1, 32, 0, s>>>(order, total, ctx->g_lo, ctx->g_hi, total + 2);
+    ctx->stats.kernel_launches += 5;
+    const GraphKeys gk = graph_keys(ctx);
+    if (edges) {
+        graph_gc_count_k<true><<<nb_lists, GRAPH_NT, 0, s>>>(nt, ctx->d_ghead, ctx->d_pool, gk, ctx->d_gdeps, ctx->d_ggen, blk);
+        graph_scan_k<<<1, 1024, 0, s>>>(nb_lists, blk, total + 1);
+        ctx->stats.kernel_launches += 2;
+    }
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(ctx->h_small + 4, total, 4 * sizeof(u32), cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    const u32 n_kept = ctx->h_small[4], live = ctx->h_small[5], own_lo = ctx->h_small[6], own_hi = ctx->h_small[7];
+    // new(h) = survivors below h, except new(n_total) = n_total: the rank whose range ends at n_total takes the freed tail
+    // (a rank with the empty range [n_total, n_total) keeps it), so the ranges still tile [0, n_total) in rank order
+    const u32 new_lo = ctx->g_lo == nt ? nt : own_lo, new_hi = ctx->g_hi == nt ? nt : own_hi;
+    const u32 n_own = own_hi - own_lo;
+    const u32 cap = std::max(ctx->cap_handles, (n_own + 1023u) & ~1023u);
+    if (cap) {
+        CU(key.grow(cap, s, false, 0));
+        CU(prio.grow(cap, s, false, 0));
+    }
+    if (n_kept) {
+        shard_compact_gather_k<<<(n_kept + 255) / 256, 256, 0, s>>>(n_kept, order, ctx->d_gvalid, ctx->d_gdeps, ctx->d_ggen,
+                                                                    ctx->g_lo, ctx->n_handles, own_lo, own_hi, ctx->d_key,
+                                                                    ctx->d_prio, gvalid, gdeps, ggen, key, prio, new_of_old);
+        ctx->stats.kernel_launches++;
+    }
+    if (edges) {
+        graph_gc_move_k<true, true><<<nb_lists, GRAPH_NT, 0, s>>>(nt, ctx->d_ghead, ctx->d_pool, pool, gk, ctx->d_gdeps,
+                                                                   ctx->d_ggen, blk, new_of_old, ghead);
+        ctx->stats.kernel_launches++;
+    }
+    CU(cudaGetLastError());
+    ctx->g_new_ready.resize(n_kept);
+    if (n_kept) CU(cudaMemcpyAsync(ctx->g_new_ready.data(), order, (size_t)n_kept * 4, cudaMemcpyDeviceToHost, s));
+    CU(cudaStreamSynchronize(s));
+    ctx->d_gvalid = std::move(gvalid);
+    ctx->d_gdeps = std::move(gdeps);
+    ctx->d_ggen = std::move(ggen);
+    ctx->d_ghead = std::move(ghead);
+    ctx->d_key = std::move(key);
+    ctx->d_prio = std::move(prio);
+    ctx->cap_handles = cap;
+    if (edges) {
+        ctx->d_pool = std::move(pool);
+        ctx->pool_used = live;
+    }
+    ctx->n_handles = n_own;
+    ctx->stats.n_handles = n_own;
+    ctx->g_lo = new_lo;
+    ctx->g_hi = new_hi;
+    range[0] = new_lo;
+    range[1] = new_hi;
+    return HQS_OK;
+}
 }  // namespace
 
 extern "C" {
@@ -1944,6 +2030,43 @@ int hqs_handles_compact(hqs_ctx* ctx, uint32_t n_keep, const uint32_t* keep, con
     }
     if (old_of_new) *old_of_new = ctx->g_new_ready.data();
     if (n_kept) *n_kept = (u32)ctx->g_new_ready.size();
+    return HQS_OK;
+}
+
+int hqs_shard_graph_compact(hqs_ctx* ctx, uint32_t n_keep, const uint32_t* keep, const uint32_t** old_of_new,
+                            uint32_t* n_kept, uint32_t new_range[2]) {
+    if (!ctx) return HQS_E_INVALID;
+    ctx->g_new_ready.clear();
+    if (old_of_new) *old_of_new = ctx->g_new_ready.data();
+    if (n_kept) *n_kept = 0;
+    if (new_range) {
+        new_range[0] = ctx->g_lo;
+        new_range[1] = ctx->g_hi;
+    }
+    if (int rc = shard_graph_mode_check(ctx, "hqs_shard_graph_compact")) return rc;
+    if (n_keep && !keep) return fail(ctx, HQS_E_INVALID, "null keep array");
+    for (u32 i = 0; i < n_keep; ++i)
+        if (keep[i] >= ctx->g_total)
+            return fail(ctx, HQS_E_INVALID, "keep handle %u >= n_total %u (nothing was compacted)", keep[i], ctx->g_total);
+    if (!ctx->g_total) return HQS_OK;
+    u32 range[2];
+    const int rc = shard_graph_outcome(ctx, [&]() -> int {
+        CU(cudaSetDevice(ctx->device));
+        if (int r = ensure_push_staging(ctx, n_keep)) return r;
+        if (n_keep) CU(cudaMemcpyAsync(ctx->d_push_task, keep, (size_t)n_keep * 4, cudaMemcpyHostToDevice, ctx->stream));
+        return shard_graph_compact_impl(ctx, n_keep, range);
+    }());
+    if (rc) {
+        ctx->g_new_ready.clear();
+        cudaStreamSynchronize(ctx->stream);       // the caller may free keep as soon as we return
+        return rc;
+    }
+    if (old_of_new) *old_of_new = ctx->g_new_ready.data();
+    if (n_kept) *n_kept = (u32)ctx->g_new_ready.size();
+    if (new_range) {
+        new_range[0] = range[0];
+        new_range[1] = range[1];
+    }
     return HQS_OK;
 }
 

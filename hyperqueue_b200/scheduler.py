@@ -231,6 +231,40 @@ def cancel_bookkeeping(s, h: np.ndarray, gone: np.ndarray) -> Dict[int, List[int
     return messages
 
 
+def tracked_handles(s, n: int) -> np.ndarray:
+    """The handles below n that the scheduler `s` still tracks on the host, whether or not their task is in the device table:
+    assigned to a worker, prefilled, or with a pending redirect or retract.  A handle compaction must keep them (int64, may
+    repeat)."""
+    tracked = np.zeros(0, dtype=np.int64)
+    if n:
+        m = min(n, s._task_worker.shape[0])
+        tracked = np.nonzero((s._task_worker[:m] >= 0) | (s._pf_worker[:m] >= 0))[0]
+    extra = list(s.redirects.keys()) + list(s._retracting_from.keys())
+    return np.concatenate([tracked, np.asarray(extra, dtype=np.int64)])
+
+
+def renumber_host_mirror(s, kept: np.ndarray) -> None:
+    """After a handle compaction: the scheduler `s`'s handle kept[i] (ascending, int64) is now handle i.  The per-handle host
+    arrays and the redirect and retract maps follow; the slots past the survivors read as never used.  The arrays must
+    already hold every kept handle."""
+    def remap(a: np.ndarray, fill) -> np.ndarray:
+        out = np.full_like(a, fill)
+        out[: kept.size] = a[kept]
+        return out
+
+    s._task_class = remap(s._task_class, 0)
+    s._task_worker = remap(s._task_worker, -1)
+    s._task_variant = remap(s._task_variant, 0)
+    s._task_prio = remap(s._task_prio, 0)
+    s._pf_worker = remap(s._pf_worker, -1)
+
+    def new_of(t: int) -> int:
+        return int(np.searchsorted(kept, t))
+
+    s.redirects = {new_of(t): v for t, v in s.redirects.items()}
+    s._retracting_from = {new_of(t): v for t, v in s._retracting_from.items()}
+
+
 def query_workers(worker_totals: np.ndarray, remaining_s: Optional[np.ndarray] = None,
                   min_utilization: Optional[np.ndarray] = None) -> Tuple[np.ndarray, np.ndarray]:
     """The fake-worker array of a what-if query (new_worker_query): worker ids 0..n-1, time limits in seconds (inf = none)
@@ -663,12 +697,7 @@ class GpuScheduler:
         with the table.  Returns old_of_new: the old handle of each new handle, ascending; the caller renumbers its own
         handles with it (np.searchsorted(old_of_new, old) for a survivor)."""
         n = int(self._lib_stats().n_handles)
-        tracked = np.zeros(0, dtype=np.int64)
-        if n:
-            m = min(n, self._task_worker.shape[0])
-            tracked = np.nonzero((self._task_worker[:m] >= 0) | (self._pf_worker[:m] >= 0))[0]
-        extra = list(self.redirects.keys()) + list(self._retracting_from.keys())
-        k = np.concatenate([tracked, np.asarray(extra, dtype=np.int64),
+        k = np.concatenate([tracked_handles(self, n),
                             np.zeros(0, np.int64) if keep is None else np.asarray(keep, dtype=np.int64).ravel()])
         k = np.ascontiguousarray(np.unique(k), dtype=np.uint32)
         ptr = C.POINTER(C.c_uint32)()
@@ -676,25 +705,8 @@ class GpuScheduler:
         self._check(self._lib.hqs_handles_compact(self._ctx, k.size, L.ptr(k) if k.size else None, C.byref(ptr),
                                                   C.byref(nk)))
         old_of_new = np.ctypeslib.as_array(ptr, shape=(nk.value,)).copy() if nk.value else np.zeros(0, dtype=np.uint32)
-        kept = old_of_new.astype(np.int64)
         self._grow_tasks(n)
-
-        def remap(a: np.ndarray, fill) -> np.ndarray:
-            out = np.full_like(a, fill)
-            out[: kept.size] = a[kept]
-            return out
-
-        self._task_class = remap(self._task_class, 0)
-        self._task_worker = remap(self._task_worker, -1)
-        self._task_variant = remap(self._task_variant, 0)
-        self._task_prio = remap(self._task_prio, 0)
-        self._pf_worker = remap(self._pf_worker, -1)
-
-        def new_of(t: int) -> int:
-            return int(np.searchsorted(old_of_new, t))
-
-        self.redirects = {new_of(t): v for t, v in self.redirects.items()}
-        self._retracting_from = {new_of(t): v for t, v in self._retracting_from.items()}
+        renumber_host_mirror(self, old_of_new.astype(np.int64))
         return old_of_new
 
     def graph_debug(self) -> np.ndarray:

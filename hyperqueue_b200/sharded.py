@@ -34,7 +34,9 @@ task of any rank carries it.
 Task graphs (ShardedScheduler.graph_init, then submit_tasks / graph_tasks_finished / graph_cancel_tasks): the graph is
 replicated on every rank (hqs_shard_graph_init) and every rank makes every graph call with the same GLOBAL arguments, runs
 the same propagation, writes the keys it owns and returns the handles it owns.  No graph data moves between ranks; the only
-collective is the free-vector all-reduce that finishing and cancelling already need.
+collective is the free-vector all-reduce that finishing and cancelling already need.  ShardedScheduler.compact_handles retires
+the handles of forgotten tasks the same way: every rank renumbers the replicated graph alike and keeps its own tasks, and the
+ranks' ranges shrink in place.
 """
 from __future__ import annotations
 
@@ -46,7 +48,8 @@ import torch
 import torch.distributed as dist
 
 from . import _lib as L
-from .scheduler import WorkerTaskMapping, apply_tick_records, cancel_bookkeeping, query_workers, return_resources
+from .scheduler import (WorkerTaskMapping, apply_tick_records, cancel_bookkeeping, query_workers, renumber_host_mirror,
+                        return_resources, tracked_handles)
 
 
 def shard_exchange(counts_local: torch.Tensor, rank: int, world: int,
@@ -388,6 +391,53 @@ class ShardedScheduler:
         msgs = cancel_bookkeeping(s, self._mine(h), gone.astype(np.int64) - self.lo)
         self._sum_free_change(before)
         return gone, {wid: [t + self.lo for t in lst] for wid, lst in msgs.items()}
+
+    def compact_handles(self, keep=None) -> np.ndarray:
+        """Retires the handles of forgotten tasks over the sharded graph (hqs_shard_graph_compact), the counterpart of
+        GpuScheduler.compact_handles.  Every rank calls it with the same arguments and gets the same old_of_new: the old
+        GLOBAL handle of each new global handle, ascending (np.searchsorted(old_of_new, old) renumbers a survivor).
+        A handle survives if its task is in the replicated graph, if any rank still tracks it on the host (assigned to a
+        worker, prefilled, with a pending redirect or retract, or a started prefilled task that left the graph), or if it is
+        in `keep` (global handles the caller tracks).  What the ranks track is gathered in one variable-length all-gather
+        (none with world == 1), so every rank passes the same keep list.  Survivor i becomes global handle i; no key moves
+        between ranks: each rank's range [lo, hi) becomes [number of survivors below lo, number below hi), and the last rank
+        also takes the freed tail up to n_total.  This rank's host mirror, redirects and retracts are renumbered, and lo / hi
+        follow the new range.
+        Intake: new tasks carry higher TaskIds than every survivor, so they get the handles of the freed tail and all land on
+        the last rank, until the caller compacts again or sets up a new sharded graph.  (Fixed blocks already put a stream of
+        TaskId-ordered submits on one rank at a time; ranges are not rebalanced by moving keys.)"""
+        s = self.s
+        mine = np.unique(tracked_handles(s, s._task_worker.shape[0])) + self.lo
+        k = np.concatenate([self._all_gather_handles(mine),
+                            np.zeros(0, np.int64) if keep is None else np.asarray(keep, dtype=np.int64).ravel()])
+        k = np.ascontiguousarray(np.unique(k), dtype=np.uint32)
+        ptr = C.POINTER(C.c_uint32)()
+        nk = C.c_uint32(0)
+        rng = np.zeros(2, dtype=np.uint32)
+        s._check(s._lib.hqs_shard_graph_compact(s._ctx, k.size, L.ptr(k) if k.size else None, C.byref(ptr), C.byref(nk),
+                                                L.ptr(rng)))
+        old_of_new = np.ctypeslib.as_array(ptr, shape=(nk.value,)).copy() if nk.value else np.zeros(0, dtype=np.uint32)
+        a, b = np.searchsorted(old_of_new, [self.lo, self.hi])
+        kept = old_of_new[a:b].astype(np.int64) - self.lo          # this rank's survivors, old local handles
+        if kept.size:
+            s._grow_tasks(int(kept[-1]) + 1)
+        renumber_host_mirror(s, kept)
+        self.lo, self.hi = int(rng[0]), int(rng[1])
+        return old_of_new
+
+    def _all_gather_handles(self, mine: np.ndarray) -> np.ndarray:
+        """The concatenation over the ranks of each rank's int64 handle list `mine` (lists of any length)."""
+        if self.world == 1:
+            return np.asarray(mine, dtype=np.int64)
+        dev = self.device if dist.get_backend(self.group) == "nccl" else torch.device("cpu")
+        sizes = [torch.zeros(1, dtype=torch.int64, device=dev) for _ in range(self.world)]
+        dist.all_gather(sizes, torch.tensor([mine.size], dtype=torch.int64, device=dev), group=self.group)
+        sizes = [int(x.item()) for x in sizes]
+        buf = torch.zeros(max(max(sizes), 1), dtype=torch.int64)
+        buf[: mine.size] = torch.from_numpy(np.asarray(mine, dtype=np.int64))
+        parts = [torch.zeros_like(buf, device=dev) for _ in range(self.world)]
+        dist.all_gather(parts, buf.to(dev), group=self.group)
+        return np.concatenate([p.cpu().numpy()[:n] for p, n in zip(parts, sizes)])
 
     def _sum_free_change(self, before: np.ndarray) -> None:
         """Returning resources only adds to a free vector: the per-worker change (>= 0, below the worker's total) is summed

@@ -283,6 +283,35 @@ int hqs_shard_graph_finished(hqs_ctx* ctx, uint32_t n, const uint32_t* task, con
 int hqs_shard_graph_cancel(hqs_ctx* ctx, uint32_t n, const uint32_t* task, const uint32_t** cancelled, uint32_t* n_cancelled);
 int hqs_shard_graph_remove(hqs_ctx* ctx, uint32_t n, const uint32_t* task);
 
+/* hqs_handles_compact over a sharded graph: every rank renumbers the replicated graph alike and keeps its own tasks.  It reads
+ * like hqs_handles_compact, with global handles, and no key moves between ranks.
+ * Survivors: every global handle whose replicated graph VALID bit is set, plus the GLOBAL handles named in keep[0 .. n_keep)
+ * (any order, repeats allowed).  The survivor set is computed from replicated state only, so every rank must pass the same
+ * keep list (ShardedScheduler.compact_handles gathers what each rank tracks).
+ * Renumbering: survivor i, in ascending old handle, becomes global handle i.  *old_of_new points to the *n_kept old handles,
+ * ascending, the same list on every rank, in the buffer hqs_graph_finished uses, valid until the next call on the context.
+ * New ranges: with new(h) = the number of survivors below h, and new(n_total) = n_total, a rank that owned [lo, hi) now owns
+ * [new(lo), new(hi)), written to new_range[0..1] (which may be NULL).  So the rank whose range ends at n_total (the last rank)
+ * owns [new(lo), n_total), the freed tail [n_kept, n_total) included, the ranges still tile [0, n_total) in rank order (the
+ * order the global rank inside a group depends on), and every survivor's key stays on the rank that owns it.  n_total is
+ * unchanged; new tasks, numbered after the survivors, land on the last rank.
+ * What moves with a survivor on every rank: its graph VALID bit, dependency count, incarnation and consumer list, with the
+ * consumers renumbered; an edge whose consumer no longer waits on the edge's incarnation is dropped.  On its owner only: its
+ * key verbatim (READY, DONE, VALID and PREFILLED bits, level and class) and its priority, now at new(h) - new(lo).  The rank's
+ * n_handles (and hqs_stats.n_handles) becomes its own survivor count (the last rank counts up to n_kept, not n_total).
+ * Unchanged: the level table, the class table, the prefill configuration and mask, the exchange buffers and the peer-to-peer
+ * sequence state.  The key table's capacity is kept (or grown to the own survivor count), and the last rank's table grows into
+ * the tail as pushes reach it.
+ * Rejections leave every rank unchanged and happen alike on every rank: HQS_E_INVALID for a keep entry >= n_total or
+ * keep == NULL with n_keep > 0; HQS_E_STATE where the sharded graph calls refuse (no hqs_shard_graph_init, which includes a
+ * sharded ready set without a graph, a replica marked failed, a pending tick or query).  HQS_E_CUDA marks the replica failed
+ * like every other sharded graph call; the rank's own arrays stay as they were (fresh arrays are swapped in only at the end).
+ * hqs_handles_compact still returns HQS_E_STATE on a sharded graph context.
+ * At most nine kernel launches whatever n_total is; the call synchronises with the host twice (the survivor count and the
+ * new ranges, then the copy of *old_of_new). */
+int hqs_shard_graph_compact(hqs_ctx* ctx, uint32_t n_keep, const uint32_t* keep, const uint32_t** old_of_new,
+                            uint32_t* n_kept, uint32_t new_range[2]);
+
 /* One scheduler tick over the current ready set (replaces run_scheduling_solver + the task-selection
  * half of create_task_mapping).
  *   workers[n_workers]            ascending worker_id
