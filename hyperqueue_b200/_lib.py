@@ -70,7 +70,7 @@ class hqs_stats(C.Structure):
 # hqs_stats.solver_path bits (include/hqsched.h)
 HQS_PATH_WIDE, HQS_PATH_LEAN, HQS_PATH_LEAN_EXTRAS, HQS_PATH_GENERAL = 0x01, 0x02, 0x04, 0x08
 HQS_PATH_PACKED, HQS_PATH_MU_RESTART, HQS_PATH_CLASSES_GLOBAL, HQS_PATH_REM_GLOBAL = 0x10, 0x20, 0x40, 0x80
-HQS_PATH_EMIT_STAGED = 0x100
+HQS_PATH_EMIT_STAGED, HQS_PATH_GROUPS_GLOBAL, HQS_PATH_BLOCKED_GLOBAL, HQS_PATH_COUNTS_GLOBAL = 0x100, 0x200, 0x400, 0x800
 
 
 worker_dtype = np.dtype([("worker_id", "<u4"), ("flags", "<u4"), ("remaining_time_ms", "<u8"),

@@ -30,6 +30,7 @@ constexpr u32 BLK_PACK = 1, BLK_RESTART = 2, BLK_END = 3, BLK_PREFILL = 4, BLK_W
 constexpr u32 TF_COUNT = 1, TF_EMIT = 2, TF_PACK = 4, TF_NO_REFRESH = 8, TF_NO_WIDE = 16;   // TF_NO_REFRESH / TF_NO_WIDE: measuring aids (HQS_DEBUG_NO_REFRESH, HQS_DEBUG_NO_WIDE)
 constexpr u32 WIDE_MAX_GROUP = 0x03FFFFFFu;   // largest group the wide first-fit handles (32-bit prefix sums)
 constexpr u32 SM_NONE = 0xFFFFFFFFu;
+constexpr u32 GLIST_GLOBAL_WORDS = 4 * HQS_MAX_GROUPS;   // group list in global memory: glist [2][G], gcl [G], kk [G]
 constexpr u32 PF_SEG_CAP = 1u << 18;  // prefill segments (eligible workers summed over classes) per tick
 constexpr u32 MU_MAX_PASSES = 8;      // restarts of the min-utilisation rule before the remaining violators are dropped
 
@@ -55,9 +56,10 @@ constexpr int TR_EMIT_CMD = 0, TR_EMIT_STAGED = 1, TR_EMIT_FILTER = 2, TR_EMIT_F
 
 // offsets into the solver CTA's dynamic shared memory (SM_NONE: the array stays in global memory)
 struct TickSmem {
-    u32 fr, rem, unt, remtime, excl, touch, td, frontier, noresv, glist, gcl;     // always staged
+    u32 fr, rem, unt, remtime, excl, touch, td, frontier, noresv; // always staged
+    u32 glist, gcl;                                                // staged unless the mandatory arrays do not fit with them
     u32 classes, vorder, blocked, bef, loc;                        // optional
-    u32 kk, top, pflvl;                                            // proactive filling only
+    u32 kk, top, pflvl;                                            // proactive filling only (kk: staged with glist)
 };
 
 struct TickArgs {
@@ -95,6 +97,7 @@ struct TickArgs {
     hqs_assignment* out;
     u32 out_cap;
     u32* rem_scratch;        // [W][RT] u64 as u32 pairs: narrow remainders when they do not fit shared memory
+    u32* glist_glob;         // [GLIST_GLOBAL_WORDS]: the group list when it does not fit shared memory (sm.glist == SM_NONE)
     // proactive filling (mapping.rs:156-230); pf_shift == 0: off.  With it on, every (level, class) splits into two groups,
     // waiting tasks first, prefilled ones second (take_tasks, taskqueue.rs:320-355): g = (level * Q + class) * 2 + prefilled
     u32 pf_shift, pf_reserve, pf_max;
@@ -707,8 +710,10 @@ __device__ void solver_cta(const TickArgs& a, unsigned char* smem) {
     uint8_t* s_noresv = smem + a.sm.noresv;                                            // [Q] no worker can be reserved for the class any more
     unsigned short* s_td = reinterpret_cast<unsigned short*>(smem + a.sm.td);          // [W] tried | dead << 8 of the current group
     unsigned short* s_front = reinterpret_cast<unsigned short*>(smem + a.sm.frontier); // [Q] first tile that may have room
-    uint2* s_glist = reinterpret_cast<uint2*>(smem + a.sm.glist);                      // [L*Q] (group, count)
-    u32* s_gcl = reinterpret_cast<u32*>(smem + a.sm.gcl);                              // [L*Q] class | level << 16
+    // the group list: shared memory, or global memory when the mandatory arrays do not fit with it (read by this CTA only)
+    const bool glist_sm = a.sm.glist != SM_NONE;
+    uint2* s_glist = glist_sm ? reinterpret_cast<uint2*>(smem + a.sm.glist) : reinterpret_cast<uint2*>(a.glist_glob);   // [L*Q] (group, count)
+    u32* s_gcl = glist_sm ? reinterpret_cast<u32*>(smem + a.sm.gcl) : a.glist_glob + 2 * HQS_MAX_GROUPS;             // [L*Q] class | level << 16
     // narrow remainders (exact amount = fr * gscale + rem): shared memory when they fit, else global scratch
     u64* p_rem = NARROW ? (a.sm.rem != SM_NONE ? reinterpret_cast<u64*>(smem + a.sm.rem) : reinterpret_cast<u64*>(a.rem_scratch)) : nullptr;
     const Cls* classes = a.sm.classes != SM_NONE ? reinterpret_cast<const Cls*>(smem + a.sm.classes) : reinterpret_cast<const Cls*>(a.classes);
@@ -716,7 +721,8 @@ __device__ void solver_cta(const TickArgs& a, unsigned char* smem) {
     const uint8_t* blocked = a.blocked ? (a.sm.blocked != SM_NONE ? smem + a.sm.blocked : a.blocked) : nullptr;
     u32* s_bef = a.sm.bef != SM_NONE ? reinterpret_cast<u32*>(smem + a.sm.bef) : nullptr;
     u32* s_loc = a.sm.loc != SM_NONE ? reinterpret_cast<u32*>(smem + a.sm.loc) : nullptr;
-    u32* s_kk = a.pf_shift ? reinterpret_cast<u32*>(smem + a.sm.kk) : nullptr;          // [L*Q*2] tasks assigned per list entry (prefill)
+    u32* s_kk = a.pf_shift ? (glist_sm ? reinterpret_cast<u32*>(smem + a.sm.kk) : a.glist_glob + 3 * HQS_MAX_GROUPS)
+                           : nullptr;                                                  // [L*Q*2] tasks assigned per list entry (prefill)
     u32* s_top = a.pf_shift ? reinterpret_cast<u32*>(smem + a.sm.top) : nullptr;        // [Q] best level with waiting tasks left
     u32* s_pflvl = a.pf_shift ? reinterpret_cast<u32*>(smem + a.sm.pflvl) : nullptr;    // [Q] level of the class's prefilled tasks
 
@@ -1477,7 +1483,9 @@ __device__ void solver_cta(const TickArgs& a, unsigned char* smem) {
     u32 n_assigned = 0, n_segments = 0, n_visits = 0, n_fast = 0;
     long long t_pack = 0, t_general = 0;      // cycles inside pack commands / the general first-fit loop (hqs_debug_read)
     // HQS_PATH_* bits of the header (hqs_stats.solver_path): where the solve's data lives, then the loops the solver warp ran
-    u32 path = (a.sm.classes == SM_NONE ? HQS_PATH_CLASSES_GLOBAL : 0u) | (NARROW && a.sm.rem == SM_NONE ? HQS_PATH_REM_GLOBAL : 0u);
+    u32 path = (a.sm.classes == SM_NONE ? HQS_PATH_CLASSES_GLOBAL : 0u) | (NARROW && a.sm.rem == SM_NONE ? HQS_PATH_REM_GLOBAL : 0u) |
+               (glist_sm ? 0u : HQS_PATH_GROUPS_GLOBAL) | (a.blocked && a.sm.blocked == SM_NONE ? HQS_PATH_BLOCKED_GLOBAL : 0u) |
+               ((a.x_world || a.before_ext) && a.sm.bef == SM_NONE ? HQS_PATH_COUNTS_GLOBAL : 0u);
 #ifdef HQS_TRACE
     // measuring build (tools/trace_build.sh): cycle sums of the sections of the lean loop replace the phase stamps
     u32 tr_top = 0, tr_rec = 0, tr_cyc[4] = {0, 0, 0, 0}, tr_n[4] = {0, 0, 0, 0}, tr_fit = 0, tr_load = 0;   // visit kinds: dead tile, fall, scan (tile exhausted), scan (group ends)

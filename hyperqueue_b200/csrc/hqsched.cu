@@ -122,6 +122,7 @@ struct TickBuffers {
     Buf<TickSync> sync;
     Buf<u64> pk_fr; Buf<u32> pk_quota, pk_taken, pk_cand, pk_meta;
     Buf<u32> rem_scratch; Buf<uint8_t> excl;
+    Buf<u32> glist;                           // [4][HQS_MAX_GROUPS] the solver's group list when it does not fit shared memory
     Buf<u32> pf_cum, pf_wk;                   // [PF_SEG_CAP] prefill segments
     Buf<unsigned char, Mem::Mapped> h_hdr;    // TickHeaderOut + free_after, written by the kernel
 };
@@ -471,6 +472,7 @@ int ensure_tick_buffers(hqs_ctx* ctx, u32 G, u32 P, u32 W, u32 out_cap) {
         CU(b.pk_meta.grow(2, s));
         CU(b.rem_scratch.grow(wr * sizeof(u64) / sizeof(u32), s));
         CU(b.excl.grow(HQS_MAX_WORKERS, s));
+        CU(b.glist.grow((size_t)GLIST_GLOBAL_WORDS, s));
         CU(b.pf_cum.grow(PF_SEG_CAP, s));
         CU(b.pf_wk.grow(PF_SEG_CAP, s));
         CU(b.h_hdr.grow(sizeof(TickHeaderOut) + wr * 8, s, false, 0));
@@ -711,6 +713,7 @@ TickArgs base_args(hqs_ctx* ctx, const TickGeom& t, u32 W, const TickLayout& lay
     a.hdr_host = reinterpret_cast<TickHeaderOut*>(tb.h_hdr.dev());
     a.out = ctx->d_out;
     a.rem_scratch = tb.rem_scratch;
+    a.glist_glob = tb.glist;
     a.sync = tb.sync;
     a.pk.fr = tb.pk_fr; a.pk.quota = tb.pk_quota; a.pk.taken = tb.pk_taken;
     a.pk.cand = tb.pk_cand; a.pk.meta = tb.pk_meta;
@@ -721,25 +724,37 @@ TickArgs base_args(hqs_ctx* ctx, const TickGeom& t, u32 W, const TickLayout& lay
     return a;
 }
 
-// shared-memory layout of the solver CTA: mandatory arrays first, then the optional ones while they fit
+// shared-memory layout of the solver CTA: mandatory arrays first, then the optional ones while they fit.  The group list
+// (glist, gcl and, with proactive filling, kk: 12 or 16 B per entry) is mandatory unless the other mandatory arrays and it
+// do not fit together (many workers x wide amounts x thousands of groups); then it lives in TickBuffers::glist, and every
+// tick that fits keeps the layout it always had.
 size_t solver_layout(const hqs_ctx* ctx, TickArgs& a, size_t budget, bool sharded) {
     const u32 W = a.W, Q = a.Q, RT = ctx->RT;
     const size_t at = ctx->tick_narrow ? 4 : 8;
     const u32 n_pos = (a.L * Q) << a.pf_shift;
     size_t o = 0;
     auto put = [&](size_t bytes) { const size_t at_ = o; o = (o + bytes + 15) & ~size_t(15); return (u32)at_; };
-    a.sm.fr = put((size_t)W * RT * at);
-    a.sm.unt = put((size_t)W * 4);
-    a.sm.remtime = put((size_t)W * 8);
-    a.sm.excl = put(W);
-    a.sm.touch = put(W);
-    a.sm.td = put((size_t)W * 2);
-    a.sm.frontier = put((size_t)Q * 2);
-    a.sm.noresv = put(Q);
-    a.sm.glist = put((size_t)n_pos * 8);
-    a.sm.gcl = put((size_t)n_pos * 4);
-    a.sm.kk = a.sm.top = a.sm.pflvl = SM_NONE;
-    if (a.pf_shift) { a.sm.kk = put((size_t)n_pos * 4); a.sm.top = put((size_t)Q * 4); a.sm.pflvl = put((size_t)Q * 4); }
+    auto mandatory = [&](bool groups) {
+        o = 0;
+        a.sm.fr = put((size_t)W * RT * at);
+        a.sm.unt = put((size_t)W * 4);
+        a.sm.remtime = put((size_t)W * 8);
+        a.sm.excl = put(W);
+        a.sm.touch = put(W);
+        a.sm.td = put((size_t)W * 2);
+        a.sm.frontier = put((size_t)Q * 2);
+        a.sm.noresv = put(Q);
+        a.sm.glist = groups ? put((size_t)n_pos * 8) : SM_NONE;
+        a.sm.gcl = groups ? put((size_t)n_pos * 4) : SM_NONE;
+        a.sm.kk = a.sm.top = a.sm.pflvl = SM_NONE;
+        if (a.pf_shift) {
+            if (groups) a.sm.kk = put((size_t)n_pos * 4);
+            a.sm.top = put((size_t)Q * 4);
+            a.sm.pflvl = put((size_t)Q * 4);
+        }
+    };
+    mandatory(true);
+    if (o > budget) mandatory(false);
     auto opt = [&](size_t bytes, bool wanted) -> u32 {
         if (!wanted || o + bytes + 16 > budget) return SM_NONE;
         return put(bytes);

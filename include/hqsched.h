@@ -125,6 +125,11 @@ typedef struct {
                                           memory; clear on an emitting tick: one pass per task (large group counts,
                                           ticks with prefill records, HQS_DEBUG_EMIT_PER_TASK; in a sharded tick this
                                           is the rank's own prefill records, so the bit can differ between ranks)  */
+#define HQS_PATH_GROUPS_GLOBAL 0x200u  /* the solver's group list did not fit shared memory next to the worker state (many
+                                          workers x wide amounts x thousands of groups) and lives in global memory    */
+#define HQS_PATH_BLOCKED_GLOBAL 0x400u /* the blocked mask did not fit shared memory and was read from global          */
+#define HQS_PATH_COUNTS_GLOBAL 0x800u  /* sharded tick: the per-group counts of this rank and of the lower ranks did not
+                                          fit shared memory and were read from global                                  */
 
 int hqs_abi_version(void);
 

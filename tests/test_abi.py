@@ -99,19 +99,29 @@ def test_cpp_shim_builds_and_exports_the_reference_interface(lib):
 
 
 def test_solver_shared_memory_budget(lib):
-    """Every instance of the tick kernel must leave room for its worst-case MANDATORY dynamic shared memory (1024 workers
-    x 16 resource slots x 8 B of free amounts + per-worker words + 4096 group-list entries: ~200 KB) inside the 227 KB
-    a CTA may use — otherwise a tick fails on the device, which the CPU-only box would not notice."""
+    """The solver CTA's dynamic shared memory may be min(227 KB - the kernel's static shared memory, 216 KB) (hqs_create).
+    Its mandatory arrays without the group list, which moves to global memory when it does not fit next to them, must fit
+    that budget at every corner of the documented limits (HQS_MAX_WORKERS, 16 resource slots, u32 / u64 amounts, proactive
+    filling on / off, HQS_MAX_CLASSES, HQS_MAX_GROUPS), or a tick there fails with HQS_E_LIMIT on every call."""
     import subprocess
     from hyperqueue_b200 import _lib
     out = subprocess.run(["cuobjdump", "-res-usage", _lib.LIB_PATH], capture_output=True, text=True).stdout
     statics = [int(m) for blk in re.findall(r"Function [^\n]*tick_k[^\n]*\n[^\n]*", out) for m in re.findall(r"SHARED:(\d+)", blk)]
     assert len(statics) == 6
-    # mandatory solver arrays: free amounts [W][RT], per-worker words, per-class words, the group list (12 B per entry).
-    # Largest supported corners: 1024 workers x 16 wide resource slots with 4096 list entries, and 8192 entries
-    # (HQS_MAX_GROUPS) with <= 8 resource slots; a tick beyond both fails with HQS_E_LIMIT before it is launched
-    for W, RT, at, Q, n_pos in [(1024, 16, 8, 4096, 4096), (1024, 8, 8, 4096, 8192), (1024, 16, 4, 4096, 8192)]:
-        worst_mandatory = W * RT * at + W * (4 + 8 + 1 + 1 + 2) + Q * 3 + n_pos * 12 + 10 * 16
-        assert max(statics) + worst_mandatory <= 227 * 1024, (W, RT, at, n_pos, max(statics), worst_mandatory)
+    budget = min(227 * 1024 - max(statics), 216 * 1024)
+    assert budget == 216 * 1024                      # tests/test_gpu_smem_layout.py predicts the layout with this budget
+    up = lambda n: (n + 15) & ~15                    # solver_layout aligns every array to 16 bytes
+    for W in (1, 1024):
+        for RT in (4, 8, 16):
+            for at in (4, 8):
+                for pf in (0, 1):
+                    for Q in (1, _lib.HQS_MAX_CLASSES):
+                        # free amounts [W][RT]; unt, remtime, excl, touch, td per worker; frontier, noresv per class;
+                        # with proactive filling top and pflvl per class
+                        need = sum(up(b) for b in (W * RT * at, W * 4, W * 8, W, W, W * 2, Q * 2, Q))
+                        need += 2 * up(Q * 4) if pf else 0
+                        assert need <= budget, (W, RT, at, pf, Q, need, budget)
+    # worst corner: 1024 workers x 16 slots x u64, proactive filling, 4096 classes
+    assert need == 192_512
     # the emit step of the worker CTAs: <= 128 KB of counters (+ the group records when they fit) + the segment cache
-    assert max(statics) + 128 * 1024 + 8 * 1024 <= 227 * 1024
+    assert 128 * 1024 + 8 * 1024 <= budget
