@@ -40,6 +40,7 @@
 #include <algorithm>
 #include <cmath>
 #include <cstdarg>
+#include <cstddef>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -87,6 +88,7 @@ public:
     }
     void swap(Buf& o) noexcept { std::swap(p_, o.p_); std::swap(dev_, o.dev_); std::swap(n_, o.n_); }
     operator T*() const { return p_; }
+    T* operator->() const { return p_; }
     T* dev() const { return dev_; }
     size_t size() const { return n_; }
 
@@ -127,6 +129,29 @@ struct TickBuffers {
     Buf<unsigned char, Mem::Mapped> h_hdr;    // TickHeaderOut + free_after, written by the kernel
 };
 
+struct TickLayout {
+    size_t off_free, off_total, off_rem, off_order, off_vorder, off_mu, off_blocked, off_pfwc, bytes;
+};
+
+// the tick input upload_tick_input staged last, and what the launches read of it; only upload_tick_input writes it
+struct TickInput {
+    u32 W;
+    TickLayout lay;
+    bool blocked, pfwc;         // it has a blocked mask, a prefill mask (proactive filling: the previous tick's prefills)
+    bool min_util, any_time;    // some worker has a minimum utilisation, a time limit
+    bool narrow;                // the tick runs the narrow solver
+};
+
+// the counters the push and graph calls copy back from the device, in page-locked memory
+struct HostCounters {
+    u32 newcnt, reject;               // d_newcnt: a push's fresh priorities (hqs_tasks_finished: its newly ready tasks), rejection bits
+    u32 ready;                        // tasks a graph push made ready at once
+    u32 emitted;                      // handles graph_emit_bits emitted (newly ready or cancelled)
+    u32 kept, live, own_lo, own_hi;   // a compaction's totals: survivors, live edges, a sharded compaction's new(lo) and new(hi)
+};
+static_assert(offsetof(HostCounters, reject) == offsetof(HostCounters, newcnt) + 4 &&
+              offsetof(HostCounters, own_hi) == offsetof(HostCounters, kept) + 12, "multi-word copies land on adjacent fields");
+
 }  // namespace
 
 struct hqs_ctx {
@@ -150,8 +175,6 @@ struct hqs_ctx {
     u32 x_world = 0, x_rank = 0, x_seq = 0;
     Buf<u32> d_xall;                      // [HQS_MAX_GROUPS] sum over ranks, written by the solver
     Buf<u32> d_xbefore;                   // [HQS_MAX_GROUPS] sum over lower ranks
-    bool x_tick = false;                  // the tick being launched uses the exchange
-    bool tick_narrow = false;             // this tick runs the narrow solver
     bool force_wide = false;              // hqs_create flag bit 1: always the 64-bit solver (tests)
     u32 RT = 4;                           // resource slots of the device class layout (4, 8 or 16)
     u32 class_bytes = 0;                  // sizeof(ClassT<RT>)
@@ -214,7 +237,7 @@ struct hqs_ctx {
     Buf<unsigned char> d_tickin;        // device copy of the tick input (blocked mask; everything when zero-copy is off)
     Buf<unsigned char, Mem::Mapped> h_tickin;   // the solver CTA reads the worker state from here
     bool zero_copy = true;
-    Buf<u32, Mem::Host> h_small;        // scratch (counters)
+    Buf<HostCounters, Mem::Host> h_cnt;
     Buf<u32, Mem::Host> h_pw;           // [HQS_MAX_WORKERS]: per-worker task counts of the last query
     // per-worker grouping of the records (hqs_tick_fetch_grouped); nothing of it exists until the first grouped fetch or
     // hqs_grouped_reserve
@@ -224,8 +247,8 @@ struct hqs_ctx {
     Buf<u32, Mem::Host> h_grp_off;      // mirror of the offset table
     float grp_ms = -1.f;                // device time of the last grouping (profiling on), < 0: none
     // last tick
-    u32 last_W = 0, last_G = 0, last_L = 0;
-    bool last_blocked = false;
+    TickInput staged{};
+    u32 last_G = 0, last_L = 0;
     bool tick_pending = false;          // a tick or a query has been launched and not fetched
     bool query_pending = false;         // ... and it is a query (hqs_query_fetch)
     bool own_stream = true;
@@ -443,7 +466,7 @@ void distinct_priorities(const u64* p, u32 n, std::vector<u64>& out) {
     for (size_t s = 0; s < slots.size(); ++s) if (used[s]) out.push_back(slots[s]);
 }
 
-int ensure_tick_buffers(hqs_ctx* ctx, u32 G, u32 P, u32 W, u32 out_cap) {
+int ensure_tick_buffers(hqs_ctx* ctx, u32 G, u32 P, u32 out_cap) {
     if (G > ctx->G_cap || P > ctx->P_cap || (size_t)G * P > (size_t)ctx->G_cap * ctx->P_cap) {
         const u32 ng = std::max(G, ctx->G_cap), np = std::max(P, ctx->P_cap);
         cudaStream_t s = ctx->stream;
@@ -480,13 +503,8 @@ int ensure_tick_buffers(hqs_ctx* ctx, u32 G, u32 P, u32 W, u32 out_cap) {
         ctx->sync_dirty = true;
     }
     if (out_cap > ctx->d_out.size()) CU(ctx->d_out.grow(std::max<u32>(out_cap, 1024), ctx->stream));
-    (void)W;
     return HQS_OK;
 }
-
-struct TickLayout {
-    size_t off_free, off_total, off_rem, off_order, off_vorder, off_mu, off_blocked, off_pfwc, bytes;
-};
 
 TickLayout tick_layout(u32 W, u32 R, u32 Q, bool blocked, bool pfwc = false) {
     TickLayout l;
@@ -598,9 +616,9 @@ int ensure_tickin(hqs_ctx* ctx, size_t bytes) {
 
 // Fills the pinned staging buffer with the tick's worker state and orders.  The solver CTA reads it in place (mapped
 // host memory, overlapped with the histogram of the worker CTAs); only the blocked mask, which the pack warps read
-// with scattered byte loads, is copied to the device.
+// with scattered byte loads, is copied to the device.  Records what it staged in ctx->staged.
 int upload_tick_input(hqs_ctx* ctx, u32 W, const hqs_worker* workers, const u64* free_rw, const u64* total_rw,
-                      const uint8_t* blocked, TickLayout* lay_out, bool* has_mu, bool* any_time) {
+                      const uint8_t* blocked) {
     const u32 R = ctx->R, Q = ctx->Q;
     const bool pfwc = ctx->pf_max && ctx->prefilled_W == W && ctx->prefilled_wc.size() == (size_t)W * Q;
     const TickLayout lay = tick_layout(W, R, Q, blocked != nullptr, pfwc);
@@ -621,7 +639,6 @@ int upload_tick_input(hqs_ctx* ctx, u32 W, const hqs_worker* workers, const u64*
             }
         narrow = over == 0;
     }
-    ctx->tick_narrow = narrow;
     ctx->stats.narrow_amounts = narrow ? 1 : 0;
     u64* rem = reinterpret_cast<u64*>(h + lay.off_rem);
     float* mu = reinterpret_cast<float*>(h + lay.off_mu);
@@ -638,15 +655,23 @@ int upload_tick_input(hqs_ctx* ctx, u32 W, const hqs_worker* workers, const u64*
         memcpy(h + lay.off_blocked, blocked, (size_t)W * Q);
     }
     if (pfwc) memcpy(h + lay.off_pfwc, ctx->prefilled_wc.data(), (size_t)W * Q);
-    ctx->h_small[11] = pfwc ? 1u : 0u;
     if (!ctx->zero_copy) CU(cudaMemcpyAsync(ctx->d_tickin, h, lay.bytes, cudaMemcpyHostToDevice, ctx->stream));
     else if (blocked || pfwc) CU(cudaMemcpyAsync(ctx->d_tickin + lay.off_blocked, h + lay.off_blocked, lay.bytes - lay.off_blocked, cudaMemcpyHostToDevice, ctx->stream));
-    *lay_out = lay;
-    *has_mu = mu_any;
-    *any_time = time_any;
-    ctx->h_small[9] = mu_any ? 1u : 0u;
-    ctx->h_small[10] = time_any ? 1u : 0u;
+    ctx->staged = TickInput{W, lay, blocked != nullptr, pfwc, mu_any, time_any, narrow};
     return HQS_OK;
+}
+
+// The staging step of the calls that upload a tick input, after their own argument checks: no tick pending, G within
+// HQS_MAX_GROUPS and groups_cap (~0u: no cap), tick buffers for out_cap records, then the upload.  *t: the tick's geometry.
+int stage_tick(hqs_ctx* ctx, u32 W, const hqs_worker* workers, const u64* free_rw, const u64* total_rw, const uint8_t* blocked,
+               u32 out_cap, u32 groups_cap, TickGeom* t) {
+    if (ctx->tick_pending) return fail(ctx, HQS_E_STATE, "the previous tick has not been fetched");
+    CU(cudaSetDevice(ctx->device));
+    *t = tick_geom(ctx);
+    if (t->G > HQS_MAX_GROUPS) return fail(ctx, HQS_E_LIMIT, "groups=%u > %u", t->G, HQS_MAX_GROUPS);
+    if (t->G > groups_cap) return fail(ctx, HQS_E_LIMIT, "groups=%u > n_groups_cap=%u", t->G, groups_cap);
+    if (int rc = ensure_tick_buffers(ctx, t->G, t->P, out_cap)) return rc;
+    return upload_tick_input(ctx, W, workers, free_rw, total_rw, blocked);
 }
 
 int validate_workers(hqs_ctx* ctx, u32 W, const hqs_worker* workers, const u64* free_rw, const u64* total_rw) {
@@ -683,24 +708,25 @@ const void* tick_fn(u32 RT, bool narrow) {
 #undef HQS_PICK
 }
 
-TickArgs base_args(hqs_ctx* ctx, const TickGeom& t, u32 W, const TickLayout& lay, bool blocked) {
+TickArgs base_args(hqs_ctx* ctx, const TickGeom& t) {
     TickArgs a;
     memset(&a, 0, sizeof a);
+    const TickInput& ti = ctx->staged;
+    const TickLayout& lay = ti.lay;
     const unsigned char* in = ctx->zero_copy ? ctx->h_tickin.dev() : ctx->d_tickin;
     a.free_rw = reinterpret_cast<const u64*>(in + lay.off_free);
     a.total_rw = reinterpret_cast<const u64*>(in + lay.off_total);
     a.rem_time = reinterpret_cast<const u64*>(in + lay.off_rem);
     a.order = reinterpret_cast<const u32*>(in + lay.off_order);
     a.vorder = in + lay.off_vorder;
-    a.blocked = blocked ? ctx->d_tickin + lay.off_blocked : nullptr;
-    a.min_util = ctx->h_small[9] ? reinterpret_cast<const float*>(in + lay.off_mu) : nullptr;
-    a.any_time_limit = ctx->h_small[10];
-    const bool narrow = ctx->tick_narrow;
-    a.classes = narrow ? ctx->d_classes32 : ctx->d_classes;
+    a.blocked = ti.blocked ? ctx->d_tickin + lay.off_blocked : nullptr;
+    a.min_util = ti.min_util ? reinterpret_cast<const float*>(in + lay.off_mu) : nullptr;
+    a.any_time_limit = ti.any_time;
+    a.classes = ti.narrow ? ctx->d_classes32 : ctx->d_classes;
     a.classes64 = ctx->d_classes;
     for (u32 r = 0; r < HQS_MAX_RESOURCES; ++r) a.gscale[r] = ctx->gscale[r] ? ctx->gscale[r] : 1;
-    a.W = W; a.Q = ctx->Q; a.L = t.L; a.R = ctx->R; a.G = t.G;
-    a.classes_bytes = ctx->Q * (narrow ? ctx->class_bytes32 : ctx->class_bytes);
+    a.W = ti.W; a.Q = ctx->Q; a.L = t.L; a.R = ctx->R; a.G = t.G;
+    a.classes_bytes = ctx->Q * (ti.narrow ? ctx->class_bytes32 : ctx->class_bytes);
     a.key = ctx->d_key; a.n_handles = ctx->n_handles; a.chunk = t.chunk; a.rows = t.rows; a.P = t.P; a.nbits = t.nbits;
     a.emit_warps = t.emit_warps; a.g_smem = t.g_smem; a.emit_stage = t.emit_stage;
     a.total_local = ctx->d_total;
@@ -719,7 +745,7 @@ TickArgs base_args(hqs_ctx* ctx, const TickGeom& t, u32 W, const TickLayout& lay
     a.pk.cand = tb.pk_cand; a.pk.meta = tb.pk_meta;
     a.excl_glob = tb.excl;
     a.pf_shift = ctx->pf_max ? 1 : 0; a.pf_reserve = ctx->pf_reserve; a.pf_max = ctx->pf_max;
-    a.prefilled_wc = ctx->h_small[11] ? ctx->d_tickin + lay.off_pfwc : nullptr;
+    a.prefilled_wc = ti.pfwc ? ctx->d_tickin + lay.off_pfwc : nullptr;
     a.gout2 = ctx->d_gout2; a.pf_cum = tb.pf_cum; a.pf_wk = tb.pf_wk;
     return a;
 }
@@ -730,7 +756,7 @@ TickArgs base_args(hqs_ctx* ctx, const TickGeom& t, u32 W, const TickLayout& lay
 // tick that fits keeps the layout it always had.
 size_t solver_layout(const hqs_ctx* ctx, TickArgs& a, size_t budget, bool sharded) {
     const u32 W = a.W, Q = a.Q, RT = ctx->RT;
-    const size_t at = ctx->tick_narrow ? 4 : 8;
+    const size_t at = ctx->staged.narrow ? 4 : 8;
     const u32 n_pos = (a.L * Q) << a.pf_shift;
     size_t o = 0;
     auto put = [&](size_t bytes) { const size_t at_ = o; o = (o + bytes + 15) & ~size_t(15); return (u32)at_; };
@@ -761,7 +787,7 @@ size_t solver_layout(const hqs_ctx* ctx, TickArgs& a, size_t budget, bool sharde
     };
     a.sm.classes = opt(a.classes_bytes, true);
     a.sm.vorder = opt((size_t)Q * HQS_MAX_VARIANTS, true);
-    a.sm.rem = opt((size_t)W * RT * 8, ctx->tick_narrow);
+    a.sm.rem = opt((size_t)W * RT * 8, ctx->staged.narrow);
     a.sm.blocked = opt((size_t)W * Q, a.blocked != nullptr);
     a.sm.bef = opt((size_t)n_pos * 4, sharded);
     a.sm.loc = a.sm.bef != SM_NONE ? opt((size_t)n_pos * 4, sharded) : SM_NONE;
@@ -770,11 +796,11 @@ size_t solver_layout(const hqs_ctx* ctx, TickArgs& a, size_t budget, bool sharde
     return o;
 }
 
-// Launches the tick kernel.  counts: nullptr (count inside the kernel), or host-provided totals (NCCL variant, the
-// histogram was taken by hqs_shard_count).  emit = false: what-if query (nothing is emitted or consumed).
-int launch_tick(hqs_ctx* ctx, const TickGeom& t, u32 W, const TickLayout& lay, bool blocked, const u32* d_counts_all,
-                const u32* d_before, u32 out_cap, bool emit, bool exchange) {
-    TickArgs a = base_args(ctx, t, W, lay, blocked);
+// Launches the tick kernel over the staged input.  counts: nullptr (count inside the kernel), or host-provided totals (NCCL
+// variant, the histogram was taken by hqs_shard_count).  emit = false: what-if query (nothing is emitted or consumed).
+int launch_tick(hqs_ctx* ctx, const TickGeom& t, const u32* d_counts_all, const u32* d_before, u32 out_cap, bool emit,
+                bool exchange) {
+    TickArgs a = base_args(ctx, t);
     a.out_cap = out_cap;
     static const bool no_refresh = getenv("HQS_DEBUG_NO_REFRESH") != nullptr;   // measuring aid: frontiers are not refreshed after a pack
     static const bool no_wide = getenv("HQS_DEBUG_NO_WIDE") != nullptr;         // measuring aid: plain ticks use the one-warp lean loop
@@ -787,8 +813,8 @@ int launch_tick(hqs_ctx* ctx, const TickGeom& t, u32 W, const TickLayout& lay, b
         a.x_world = ctx->x_world; a.x_rank = ctx->x_rank; a.x_seq = ctx->x_seq;
         a.x_all = ctx->d_xall; a.x_before = ctx->d_xbefore;
     }
-    const void* fn = tick_fn(ctx->RT, ctx->tick_narrow);
-    const size_t budget = ctx->smem_budget[ctx->tick_narrow ? 0 : 1];
+    const void* fn = tick_fn(ctx->RT, ctx->staged.narrow);
+    const size_t budget = ctx->smem_budget[ctx->staged.narrow ? 0 : 1];
     const size_t solver_smem = solver_layout(ctx, a, budget, exchange || d_before != nullptr);
     const size_t smem = std::max(solver_smem, t.worker_smem);
     if (smem > budget) return fail(ctx, HQS_E_LIMIT, "tick needs %zu bytes of shared memory, %zu available", smem, budget);
@@ -805,7 +831,7 @@ int launch_tick(hqs_ctx* ctx, const TickGeom& t, u32 W, const TickLayout& lay, b
     ctx->stats.kernel_launches++;
     CU(cudaGetLastError());
     if (ctx->profile) { CU(cudaEventRecord(ctx->ev[3], ctx->stream)); ctx->ev_valid = true; }
-    ctx->last_W = W; ctx->last_G = t.G; ctx->last_L = t.L;
+    ctx->last_G = t.G; ctx->last_L = t.L;
     return HQS_OK;
 }
 
@@ -860,12 +886,12 @@ int ensure_query_buffers(hqs_ctx* ctx) {
 // What-if query: the tick kernel without its emit step (nothing is emitted or consumed), then the per-worker task counts of
 // its count segments into the pinned buffer hqs_query_fetch reads.  Like a tick, the query is pending until it is fetched.
 // counts_all / exchange as for launch_tick (a query has no local share, so no ranks_before).
-int launch_query(hqs_ctx* ctx, const TickGeom& t, u32 W, const TickLayout& lay, bool blocked, const u32* d_counts_all,
-                 bool exchange) {
+int launch_query(hqs_ctx* ctx, const TickGeom& t, const u32* d_counts_all, bool exchange) {
     int rc = ensure_query_buffers(ctx);
     if (rc) return rc;
-    rc = launch_tick(ctx, t, W, lay, blocked, d_counts_all, nullptr, 0, false, exchange);
+    rc = launch_tick(ctx, t, d_counts_all, nullptr, 0, false, exchange);
     if (rc) return rc;
+    const u32 W = ctx->staged.W;
     u32* d_pw = ctx->tick.pk_quota;    // scratch (pack is over): [W] counters
     CU(cudaMemsetAsync(d_pw, 0, W * sizeof(u32), ctx->stream));
     seg_worker_totals_k<<<(t.G + 127) / 128, 128, 0, ctx->stream>>>(ctx->d_gout, t.G, ctx->tick.seg_cum, ctx->tick.seg_wv, d_pw);
@@ -882,17 +908,11 @@ int query_launch_impl(hqs_ctx* ctx, u32 n_workers, const hqs_worker* workers, co
                       const uint8_t* blocked_wcv, bool exchange) {
     int rc = validate_workers(ctx, n_workers, workers, free_rw, total_rw);
     if (rc) return rc;
-    if (ctx->tick_pending) return fail(ctx, HQS_E_STATE, "the previous tick has not been fetched");
-    CU(cudaSetDevice(ctx->device));
-    const TickGeom t = tick_geom(ctx);
-    if (t.G > HQS_MAX_GROUPS) return fail(ctx, HQS_E_LIMIT, "groups=%u > %u", t.G, HQS_MAX_GROUPS);
-    if ((rc = ensure_tick_buffers(ctx, t.G, t.P, n_workers, 1024))) return rc;
-    TickLayout lay;
-    bool has_mu, any_time;
-    if ((rc = upload_tick_input(ctx, n_workers, workers, free_rw, total_rw, blocked_wcv, &lay, &has_mu, &any_time))) return rc;
+    TickGeom t;
+    if ((rc = stage_tick(ctx, n_workers, workers, free_rw, total_rw, blocked_wcv, 1024, ~0u, &t))) return rc;
     // ticks and queries share one exchange sequence: every rank advances it in lockstep
     if (exchange) ctx->x_seq += 1;
-    return launch_query(ctx, t, n_workers, lay, blocked_wcv != nullptr, nullptr, exchange);
+    return launch_query(ctx, t, nullptr, exchange);
 }
 
 // Per-worker grouping (hqs_group.cuh).  Like the query's extras, its buffers and kernels are set up by the first grouped fetch
@@ -952,8 +972,8 @@ int tick_fetch_impl(hqs_ctx* ctx, u32 out_cap, hqs_assignment* out, u32* out_n, 
     const u32 n_rec = hdr.n_assigned + hdr.n_prefilled;           // assignments (kind 0 / 2), then prefills (kind 1)
     if (hdr.error == 3 || n_rec > out_cap || (n_rec && !out))
         return fail(ctx, HQS_E_OVERFLOW, "out_cap=%u too small for %u assignments + %u prefills", out_cap, hdr.n_assigned, hdr.n_prefilled);
-    if (free_after) memcpy(free_after, ctx->tick.h_hdr + sizeof(TickHeaderOut), (size_t)ctx->last_W * ctx->R * 8);
-    const u32 W = ctx->last_W, n_off = 2 * W + 2;
+    const u32 W = ctx->staged.W, n_off = 2 * W + 2;
+    if (free_after) memcpy(free_after, ctx->tick.h_hdr + sizeof(TickHeaderOut), (size_t)W * ctx->R * 8);
     if (worker_off) memset(worker_off, 0, n_off * sizeof(u32));
     if (n_rec && !worker_off) {
         CU(cudaMemcpyAsync(out, ctx->d_out, (size_t)n_rec * sizeof(hqs_assignment), cudaMemcpyDeviceToHost, ctx->stream));
@@ -1012,7 +1032,7 @@ int hqs_create(hqs_ctx** out, int device, uint32_t n_resources, uint32_t flags) 
     if (e == cudaSuccess) e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
     if (e == cudaSuccess) e = ctx->d_newcnt.grow(2, ctx->stream);
     if (e == cudaSuccess) e = ctx->d_newprio.grow(NEWPRIO_CAP, ctx->stream);
-    if (e == cudaSuccess) e = ctx->h_small.grow(64, ctx->stream);
+    if (e == cudaSuccess) e = ctx->h_cnt.grow(1, ctx->stream);
     {
         const void* fns[] = {(const void*)tick_k<4, u32>, (const void*)tick_k<8, u32>, (const void*)tick_k<16, u32>,
                              (const void*)tick_k<4, u64>, (const void*)tick_k<8, u64>, (const void*)tick_k<16, u64>};
@@ -1158,7 +1178,7 @@ u32 graph_bound(const hqs_ctx* ctx) { return ctx->shard_graph ? ctx->g_total : c
 
 // shared body of hqs_ready_push / hqs_ready_push_range (task == nullptr: handles first_handle .. first_handle + n - 1) and
 // hqs_graph_push (g != nullptr: the batch is also rejected if a pushed handle is VALID, and graph_link_k runs after push_k;
-// h_small[2] receives the number of tasks ready at once).  A sharded graph push passes the owned part of its batch, which
+// h_cnt->ready receives the number of tasks ready at once).  A sharded graph push passes the owned part of its batch, which
 // may be empty.
 int push_impl(hqs_ctx* ctx, u32 n, const u32* task, u32 first_handle, const u32* class_id, const u64* priority,
               const GraphBatch* g = nullptr) {
@@ -1213,22 +1233,22 @@ int push_impl(hqs_ctx* ctx, u32 n, const u32* task, u32 first_handle, const u32*
                 g->n, gtask, ctx->d_gstage, ctx->d_gstage + g->n + 1, g->e0, ctx->d_newcnt, gk, ctx->d_gdeps, ctx->d_ggen,
                 ctx->d_ghead, ctx->d_pool, ctx->d_gsmall);
         });
-        CU(cudaMemcpyAsync(ctx->h_small + 2, ctx->d_gsmall, sizeof(u32), cudaMemcpyDeviceToHost, ctx->stream));
+        CU(cudaMemcpyAsync(&ctx->h_cnt->ready, ctx->d_gsmall, sizeof(u32), cudaMemcpyDeviceToHost, ctx->stream));
         ctx->stats.kernel_launches += 2;
     }
     CU(cudaGetLastError());
-    CU(cudaMemcpyAsync(ctx->h_small, ctx->d_newcnt, 2 * sizeof(u32), cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaMemcpyAsync(&ctx->h_cnt->newcnt, ctx->d_newcnt, 2 * sizeof(u32), cudaMemcpyDeviceToHost, ctx->stream));
     // a coarse table has a bucket for every priority, so push_k reports none as fresh: the batch's priorities are
     // collected here, while the kernels run, and registered like fresh ones (the level set keeps growing, gets pruned
     // and leaves coarse mode once the live priorities fit again).  Exact-mode pushes do not take this pass.
     std::vector<u64> fresh;
     if (ctx->coarse) distinct_priorities(priority, n, fresh);
     CU(cudaStreamSynchronize(ctx->stream));
-    if (ctx->h_small[1] & 1u) return fail(ctx, HQS_E_INVALID, "a class id of the batch is >= n_classes %u (nothing was pushed)", ctx->Q);
-    if (ctx->h_small[1]) return fail(ctx, HQS_E_INVALID, "a handle of the batch is a live task (nothing was pushed)");
+    if (ctx->h_cnt->reject & 1u) return fail(ctx, HQS_E_INVALID, "a class id of the batch is >= n_classes %u (nothing was pushed)", ctx->Q);
+    if (ctx->h_cnt->reject) return fail(ctx, HQS_E_INVALID, "a handle of the batch is a live task (nothing was pushed)");
     if (n) ctx->n_handles = std::max(ctx->n_handles, max_h + 1);
     ctx->stats.n_handles = ctx->n_handles;
-    const u32 newcnt = ctx->h_small[0];
+    const u32 newcnt = ctx->h_cnt->newcnt;
     bool grew = false;
     if (ctx->coarse) {
         grew = merge_levels(ctx, fresh);
@@ -1446,9 +1466,9 @@ int hqs_tasks_finished(hqs_ctx* ctx, uint32_t n, const uint32_t* task, uint32_t*
     ctx->stats.kernel_launches++;
     CU(cudaGetLastError());
     if (n_new_ready) {
-        CU(cudaMemcpyAsync(ctx->h_small, ctx->d_newcnt, sizeof(u32), cudaMemcpyDeviceToHost, ctx->stream));
+        CU(cudaMemcpyAsync(&ctx->h_cnt->newcnt, ctx->d_newcnt, sizeof(u32), cudaMemcpyDeviceToHost, ctx->stream));
         CU(cudaStreamSynchronize(ctx->stream));
-        *n_new_ready = ctx->h_small[0];
+        *n_new_ready = ctx->h_cnt->newcnt;
     }
     return HQS_OK;
 }
@@ -1516,9 +1536,9 @@ int graph_compact(hqs_ctx* ctx, u32 n_edges) {
         graph_scan_k<<<1, 1024, 0, ctx->stream>>>(nb, ctx->d_gblk, ctx->d_gsmall + 2);
         ctx->stats.kernel_launches += 2;
         CU(cudaGetLastError());
-        CU(cudaMemcpyAsync(ctx->h_small + 4, ctx->d_gsmall + 2, sizeof(u32), cudaMemcpyDeviceToHost, ctx->stream));
+        CU(cudaMemcpyAsync(&ctx->h_cnt->live, ctx->d_gsmall + 2, sizeof(u32), cudaMemcpyDeviceToHost, ctx->stream));
         CU(cudaStreamSynchronize(ctx->stream));
-        live = ctx->h_small[4];
+        live = ctx->h_cnt->live;
     }
     const u64 want = std::max<u64>(ctx->pool_cap, 2ull * live + n_edges);
     if (want >= GRAPH_NIL) return fail(ctx, HQS_E_LIMIT, "the edge pool would need %llu slots", (unsigned long long)want);
@@ -1557,10 +1577,10 @@ int graph_prevalidate(hqs_ctx* ctx, u32 n, const u32* task, const u32* class_id,
         ctx->stats.kernel_launches += 2;
     }
     CU(cudaGetLastError());
-    CU(cudaMemcpyAsync(ctx->h_small, ctx->d_newcnt, 2 * sizeof(u32), cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaMemcpyAsync(&ctx->h_cnt->newcnt, ctx->d_newcnt, 2 * sizeof(u32), cudaMemcpyDeviceToHost, ctx->stream));
     CU(cudaStreamSynchronize(ctx->stream));
-    if (ctx->h_small[1] & 1u) return fail(ctx, HQS_E_INVALID, "a class id of the batch is >= n_classes %u (nothing was pushed)", ctx->Q);
-    if (ctx->h_small[1]) return fail(ctx, HQS_E_INVALID, "a handle of the batch is a live task (nothing was pushed)");
+    if (ctx->h_cnt->reject & 1u) return fail(ctx, HQS_E_INVALID, "a class id of the batch is >= n_classes %u (nothing was pushed)", ctx->Q);
+    if (ctx->h_cnt->reject) return fail(ctx, HQS_E_INVALID, "a handle of the batch is a live task (nothing was pushed)");
     return HQS_OK;
 }
 
@@ -1690,7 +1710,7 @@ int graph_push_impl(hqs_ctx* ctx, u32 n, const u32* task, const u32* class_id, c
     if (rc) return rc;
     ctx->pool_used += me;
     ctx->graph = true;
-    if (n_ready) *n_ready = ctx->h_small[2];
+    if (n_ready) *n_ready = ctx->h_cnt->ready;
     return HQS_OK;
 }
 
@@ -1726,9 +1746,9 @@ int graph_finished_impl(hqs_ctx* ctx, u32 n, const u32* task, const u32** new_re
     graph_emit_bits(ctx);
     ctx->stats.kernel_launches += 5;
     CU(cudaGetLastError());
-    CU(cudaMemcpyAsync(ctx->h_small + 3, ctx->d_gsmall + 1, sizeof(u32), cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaMemcpyAsync(&ctx->h_cnt->emitted, ctx->d_gsmall + 1, sizeof(u32), cudaMemcpyDeviceToHost, ctx->stream));
     CU(cudaStreamSynchronize(ctx->stream));
-    const u32 k = ctx->h_small[3];
+    const u32 k = ctx->h_cnt->emitted;
     ctx->g_new_ready.resize(k);
     if (k) {
         CU(cudaMemcpyAsync(ctx->g_new_ready.data(), ctx->d_gready, (size_t)k * 4, cudaMemcpyDeviceToHost, ctx->stream));
@@ -1777,12 +1797,12 @@ int graph_cancel_impl(hqs_ctx* ctx, u32 n, const u32* task, const u32** cancelle
     CU(cudaGetLastError());
     GraphCancelSync hs;
     CU(cudaMemcpyAsync(&hs, ctx->d_gcsync, sizeof hs, cudaMemcpyDeviceToHost, ctx->stream));
-    CU(cudaMemcpyAsync(ctx->h_small + 3, ctx->d_gsmall + 1, sizeof(u32), cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaMemcpyAsync(&ctx->h_cnt->emitted, ctx->d_gsmall + 1, sizeof(u32), cudaMemcpyDeviceToHost, ctx->stream));
     CU(cudaStreamSynchronize(ctx->stream));
     if (hs.error || !hs.done)
         return fail(ctx, HQS_E_CUDA, "a wait of the cancel marking kernel timed out (%s; %u handles marked, nothing was cancelled)",
                     hs.error == 2 ? "a work-list slot that was never written" : "the work list made no progress", hs.tail);
-    const u32 k = ctx->h_small[3];
+    const u32 k = ctx->h_cnt->emitted;
     ctx->g_new_ready.resize(k);
     if (k) {
         CU(cudaMemcpyAsync(ctx->g_new_ready.data(), ctx->d_gready, (size_t)k * 4, cudaMemcpyDeviceToHost, ctx->stream));
@@ -1840,9 +1860,9 @@ int handles_compact_impl(hqs_ctx* ctx, u32 n_keep) {
         ctx->stats.kernel_launches += 2;
     }
     CU(cudaGetLastError());
-    CU(cudaMemcpyAsync(ctx->h_small + 4, total, 2 * sizeof(u32), cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(&ctx->h_cnt->kept, total, 2 * sizeof(u32), cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
-    const u32 n_kept = ctx->h_small[4], live = ctx->h_small[5];
+    const u32 n_kept = ctx->h_cnt->kept, live = ctx->h_cnt->live;
     if (n_kept) {
         compact_gather_k<<<(n_kept + 255) / 256, 256, 0, s>>>(n_kept, order, ctx->d_key, ctx->d_prio,
                                                               graph ? (u32*)ctx->d_gdeps : nullptr, ctx->d_ggen, key, prio,
@@ -1913,9 +1933,9 @@ int shard_graph_compact_impl(hqs_ctx* ctx, u32 n_keep, u32 range[2]) {
         ctx->stats.kernel_launches += 2;
     }
     CU(cudaGetLastError());
-    CU(cudaMemcpyAsync(ctx->h_small + 4, total, 4 * sizeof(u32), cudaMemcpyDeviceToHost, s));
+    CU(cudaMemcpyAsync(&ctx->h_cnt->kept, total, 4 * sizeof(u32), cudaMemcpyDeviceToHost, s));
     CU(cudaStreamSynchronize(s));
-    const u32 n_kept = ctx->h_small[4], live = ctx->h_small[5], own_lo = ctx->h_small[6], own_hi = ctx->h_small[7];
+    const u32 n_kept = ctx->h_cnt->kept, live = ctx->h_cnt->live, own_lo = ctx->h_cnt->own_lo, own_hi = ctx->h_cnt->own_hi;
     // new(h) = survivors below h, except new(n_total) = n_total: the rank whose range ends at n_total takes the freed tail
     // (a rank with the empty range [n_total, n_total) keeps it), so the ranges still tile [0, n_total) in rank order
     const u32 new_lo = ctx->g_lo == nt ? nt : own_lo, new_hi = ctx->g_hi == nt ? nt : own_hi;
@@ -2150,15 +2170,9 @@ int hqs_tick_launch(hqs_ctx* ctx, uint32_t n_workers, const hqs_worker* workers,
     if (!ctx) return HQS_E_INVALID;
     int rc = validate_workers(ctx, n_workers, workers, free_rw, total_rw);
     if (rc) return rc;
-    if (ctx->tick_pending) return fail(ctx, HQS_E_STATE, "the previous tick has not been fetched");
-    CU(cudaSetDevice(ctx->device));
-    const TickGeom t = tick_geom(ctx);
-    if (t.G > HQS_MAX_GROUPS) return fail(ctx, HQS_E_LIMIT, "groups=%u > %u", t.G, HQS_MAX_GROUPS);
-    if ((rc = ensure_tick_buffers(ctx, t.G, t.P, n_workers, out_cap))) return rc;
-    TickLayout lay;
-    bool has_mu, any_time;
-    if ((rc = upload_tick_input(ctx, n_workers, workers, free_rw, total_rw, blocked_wcv, &lay, &has_mu, &any_time))) return rc;
-    if ((rc = launch_tick(ctx, t, n_workers, lay, blocked_wcv != nullptr, nullptr, nullptr, out_cap, true, false))) return rc;
+    TickGeom t;
+    if ((rc = stage_tick(ctx, n_workers, workers, free_rw, total_rw, blocked_wcv, out_cap, ~0u, &t))) return rc;
+    if ((rc = launch_tick(ctx, t, nullptr, nullptr, out_cap, true, false))) return rc;
     ctx->tick_pending = true;
     ctx->stats.ticks++;
     return HQS_OK;
@@ -2177,8 +2191,8 @@ int hqs_tick_fetch_grouped(hqs_ctx* ctx, uint32_t out_cap, hqs_assignment* out, 
     if (!ctx->tick_pending) return fail(ctx, HQS_E_STATE, "no tick in flight");
     if (ctx->query_pending) return fail(ctx, HQS_E_STATE, "a query is in flight: fetch it with hqs_query_fetch");
     // checked before the tick is consumed: it stays fetchable
-    if (!worker_off || off_cap < 2 * ctx->last_W + 2)
-        return fail(ctx, HQS_E_INVALID, "worker_off needs 2 * n_workers + 2 = %u entries (off_cap=%u)", 2 * ctx->last_W + 2, off_cap);
+    if (!worker_off || off_cap < 2 * ctx->staged.W + 2)
+        return fail(ctx, HQS_E_INVALID, "worker_off needs 2 * n_workers + 2 = %u entries (off_cap=%u)", 2 * ctx->staged.W + 2, off_cap);
     return tick_fetch_impl(ctx, out_cap, out, out_n, free_after, worker_off);
 }
 
@@ -2239,14 +2253,15 @@ int hqs_query_fetch(hqs_ctx* ctx, uint32_t* n_would_assign, uint32_t* per_worker
     TickHeaderOut hdr;
     const int rc = wait_header(ctx, &hdr);
     if (rc) return rc;
-    if (free_after) memcpy(free_after, ctx->tick.h_hdr + sizeof(TickHeaderOut), (size_t)ctx->last_W * ctx->R * 8);
+    const u32 W = ctx->staged.W;
+    if (free_after) memcpy(free_after, ctx->tick.h_hdr + sizeof(TickHeaderOut), (size_t)W * ctx->R * 8);
     // the count segments cover every group's assigned ranks [0, k), so the per-worker counts sum to the tasks assigned over
     // all ranks; the header's n_assigned of a sharded launch is this rank's share only (the solver's local output offsets)
     u32 total = 0;
-    for (u32 w = 0; w < ctx->last_W; ++w) total += ctx->h_pw[w];
+    for (u32 w = 0; w < W; ++w) total += ctx->h_pw[w];
     ctx->stats.n_assigned = total;
     if (n_would_assign) *n_would_assign = total;
-    if (per_worker_assigned) memcpy(per_worker_assigned, ctx->h_pw, ctx->last_W * sizeof(u32));
+    if (per_worker_assigned) memcpy(per_worker_assigned, ctx->h_pw, W * sizeof(u32));
     return HQS_OK;
 }
 
@@ -2257,18 +2272,11 @@ int hqs_shard_count(hqs_ctx* ctx, uint32_t n_workers, const hqs_worker* workers,
     int rc = validate_workers(ctx, n_workers, workers, free_rw, total_rw);
     if (rc) return rc;
     if (!d_counts) return fail(ctx, HQS_E_INVALID, "null d_counts");
-    if (ctx->tick_pending) return fail(ctx, HQS_E_STATE, "the previous tick has not been fetched");
-    CU(cudaSetDevice(ctx->device));
-    const TickGeom t = tick_geom(ctx);
-    if (t.G > HQS_MAX_GROUPS) return fail(ctx, HQS_E_LIMIT, "groups=%u > %u", t.G, HQS_MAX_GROUPS);
-    if (t.G > n_groups_cap) return fail(ctx, HQS_E_LIMIT, "groups=%u > n_groups_cap=%u", t.G, n_groups_cap);
-    if ((rc = ensure_tick_buffers(ctx, t.G, t.P, n_workers, 1024))) return rc;
-    TickLayout lay;
-    bool has_mu, any_time;
-    if ((rc = upload_tick_input(ctx, n_workers, workers, free_rw, total_rw, blocked_wcv, &lay, &has_mu, &any_time))) return rc;
+    TickGeom t;
+    if ((rc = stage_tick(ctx, n_workers, workers, free_rw, total_rw, blocked_wcv, 1024, n_groups_cap, &t))) return rc;
     CU(cudaMemsetAsync(ctx->d_total, 0, (size_t)t.G * 4, ctx->stream));
     if (ctx->n_handles) {
-        TickArgs a = base_args(ctx, t, n_workers, lay, blocked_wcv != nullptr);
+        TickArgs a = base_args(ctx, t);
         count_only_k<<<std::min<u32>(t.P, ctx->sm_count * 2), TICK_THREADS, t.G * sizeof(u32), ctx->stream>>>(a);
         ctx->stats.kernel_launches++;
         CU(cudaGetLastError());
@@ -2276,8 +2284,6 @@ int hqs_shard_count(hqs_ctx* ctx, uint32_t n_workers, const hqs_worker* workers,
     CU(cudaMemsetAsync(d_counts, 0, (size_t)n_groups_cap * 4, ctx->stream));
     CU(cudaMemcpyAsync(d_counts, ctx->d_total, (size_t)t.G * 4, cudaMemcpyDeviceToDevice, ctx->stream));
     CU(cudaStreamSynchronize(ctx->stream));
-    ctx->last_W = n_workers;
-    ctx->last_blocked = blocked_wcv != nullptr;
     if (n_groups) *n_groups = t.G;
     return HQS_OK;
 }
@@ -2285,14 +2291,13 @@ int hqs_shard_count(hqs_ctx* ctx, uint32_t n_workers, const hqs_worker* workers,
 int hqs_shard_solve_emit(hqs_ctx* ctx, const uint32_t* d_counts_all, const uint32_t* d_ranks_before, uint32_t out_cap) {
     if (!ctx) return HQS_E_INVALID;
     if (!d_counts_all || !d_ranks_before) return fail(ctx, HQS_E_INVALID, "null count vectors");
-    if (!ctx->last_W) return fail(ctx, HQS_E_STATE, "hqs_shard_count has not been called");
+    if (!ctx->staged.W) return fail(ctx, HQS_E_STATE, "hqs_shard_count has not been called");
     CU(cudaSetDevice(ctx->device));
     const TickGeom t = tick_geom(ctx);
-    int rc = ensure_tick_buffers(ctx, t.G, t.P, ctx->last_W, out_cap);
+    int rc = ensure_tick_buffers(ctx, t.G, t.P, out_cap);
     if (rc) return rc;
-    // the tick input hqs_shard_count uploaded, prefill mask included (h_small[11] says whether it has one)
-    const TickLayout lay = tick_layout(ctx->last_W, ctx->R, ctx->Q, ctx->last_blocked, ctx->h_small[11] != 0);
-    if ((rc = launch_tick(ctx, t, ctx->last_W, lay, ctx->last_blocked, d_counts_all, d_ranks_before, out_cap, true, false))) return rc;
+    // over the tick input hqs_shard_count staged
+    if ((rc = launch_tick(ctx, t, d_counts_all, d_ranks_before, out_cap, true, false))) return rc;
     ctx->tick_pending = true;
     ctx->stats.ticks++;
     return HQS_OK;
@@ -2305,7 +2310,7 @@ int hqs_tick_reserve(hqs_ctx* ctx, uint32_t n_workers, uint32_t out_cap, int wit
     CU(cudaSetDevice(ctx->device));
     const TickGeom t = tick_geom(ctx);
     if (t.G > HQS_MAX_GROUPS) return fail(ctx, HQS_E_LIMIT, "groups=%u > %u", t.G, HQS_MAX_GROUPS);
-    int rc = ensure_tick_buffers(ctx, t.G, t.P, n_workers, out_cap);
+    int rc = ensure_tick_buffers(ctx, t.G, t.P, out_cap);
     if (rc) return rc;
     const TickLayout lay = tick_layout(n_workers, ctx->R, ctx->Q, with_blocked != 0, ctx->pf_max != 0);   // + the prefill mask
     if ((rc = ensure_tickin(ctx, lay.bytes))) return rc;
@@ -2381,17 +2386,11 @@ int hqs_shard_tick_launch(hqs_ctx* ctx, uint32_t n_workers, const hqs_worker* wo
     if (!ctx->x_world) return fail(ctx, HQS_E_STATE, "hqs_shard_attach has not been called");
     int rc = validate_workers(ctx, n_workers, workers, free_rw, total_rw);
     if (rc) return rc;
-    if (ctx->tick_pending) return fail(ctx, HQS_E_STATE, "the previous tick has not been fetched");
-    CU(cudaSetDevice(ctx->device));
-    const TickGeom t = tick_geom(ctx);
-    if (t.G > HQS_MAX_GROUPS) return fail(ctx, HQS_E_LIMIT, "groups=%u > %u", t.G, HQS_MAX_GROUPS);
-    if ((rc = ensure_tick_buffers(ctx, t.G, t.P, n_workers, out_cap))) return rc;
-    TickLayout lay;
-    bool has_mu, any_time;
-    if ((rc = upload_tick_input(ctx, n_workers, workers, free_rw, total_rw, blocked_wcv, &lay, &has_mu, &any_time))) return rc;
+    TickGeom t;
+    if ((rc = stage_tick(ctx, n_workers, workers, free_rw, total_rw, blocked_wcv, out_cap, ~0u, &t))) return rc;
     // every rank advances the sequence number in lockstep (one sharded tick = one exchange)
     ctx->x_seq += 1;
-    if ((rc = launch_tick(ctx, t, n_workers, lay, blocked_wcv != nullptr, nullptr, nullptr, out_cap, true, true))) return rc;
+    if ((rc = launch_tick(ctx, t, nullptr, nullptr, out_cap, true, true))) return rc;
     ctx->tick_pending = true;
     ctx->stats.ticks++;
     return HQS_OK;
@@ -2407,15 +2406,14 @@ int hqs_shard_query_launch(hqs_ctx* ctx, uint32_t n_workers, const hqs_worker* w
 int hqs_shard_query_solve(hqs_ctx* ctx, const uint32_t* d_counts_all) {
     if (!ctx) return HQS_E_INVALID;
     if (!d_counts_all) return fail(ctx, HQS_E_INVALID, "null count vector");
-    if (!ctx->last_W) return fail(ctx, HQS_E_STATE, "hqs_shard_count has not been called");
+    if (!ctx->staged.W) return fail(ctx, HQS_E_STATE, "hqs_shard_count has not been called");
     if (ctx->tick_pending) return fail(ctx, HQS_E_STATE, "the previous tick has not been fetched");
     CU(cudaSetDevice(ctx->device));
     const TickGeom t = tick_geom(ctx);
-    int rc = ensure_tick_buffers(ctx, t.G, t.P, ctx->last_W, 1024);
+    int rc = ensure_tick_buffers(ctx, t.G, t.P, 1024);
     if (rc) return rc;
-    // the tick input hqs_shard_count uploaded
-    const TickLayout lay = tick_layout(ctx->last_W, ctx->R, ctx->Q, ctx->last_blocked, ctx->h_small[11] != 0);
-    return launch_query(ctx, t, ctx->last_W, lay, ctx->last_blocked, d_counts_all, false);
+    // over the tick input hqs_shard_count staged
+    return launch_query(ctx, t, d_counts_all, false);
 }
 
 int hqs_device_result(hqs_ctx* ctx, const hqs_assignment** d_out, const uint32_t** d_out_n) {
